@@ -1,18 +1,18 @@
 #!/usr/bin/env python
 """bench.py -- decode tokens/s + p50 per-token latency of the MoE dispatch hot path, Mixtral-8x7B shapes.
 
-Contract (see task statement): `python bench.py --gpus N --steps K --warmup W [--impl reference]`
-prints ONE JSON line on rank 0.
+`python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]` prints ONE JSON line on rank 0.
 
-Workload (N=1, BASELINE.json configs[1]): Mixtral-8x7B bf16, random-init N(0,0.02^2) weights, 32 MoE layers,
-8 experts, top-2, H=4096, I=14336; decode batch 8 => T=8 tokens enter every MoE block per step; all 256
-experts HBM resident (90.2 GB).  A "step" = one pass of the hot path (router gate + softmax/top-k + permute +
-grouped gate/up GEMM with fused SwiGLU + grouped down GEMM + weighted combine) over the 32 layers for one batch
+Workload (N=1): Mixtral-8x7B bf16 MoE blocks, random-init N(0,0.02^2) weights, 8 experts, top-2, H=4096, I=14336;
+decode batch 8 => T=8 tokens enter every MoE block per step.  16 of the model's 32 MoE layers, all 128 of their experts
+HBM resident (45.1 GB): the share of Mixtral-8x7B (90 GB of experts) one 80 GB H100 holds when the model is split over
+two GPUs by layers.  A "step" = one pass of the hot path (router gate + softmax/top-k + permute +
+grouped gate/up GEMM with fused SwiGLU + grouped down GEMM + weighted combine) over the 16 layers for one batch
 of synthetic hidden states (the attention between MoE blocks is outside the path, SURVEY §8).
-  value : whole-job tokens/s with inputs resident in HBM, the 32-layer step replayed as one CUDA graph.
+  value : whole-job tokens/s with inputs resident in HBM, the 16-layer step replayed as one CUDA graph.
   e2e   : same metric through the public Python API with HOST buffers (DecodeSession.step()): the step's inputs
           are copied from pinned host memory and its outputs copied back inside the timed region; the per-layer
-          eager API (MoEEngine.forward x 32) is reported next to it.
+          eager API (MoEEngine.forward per layer) is reported next to it.
   roofline : dominant kernel = grouped gate/up GEMM (K3, 2/3 of the weight bytes), timed with CUDA events on
           its launch stream; algorithmic bytes counted from the actual routing of the timed inputs.
   cpu_baseline : the reference's CPU path on the host cores for a bounded sample (as many full-size layers as fit
@@ -20,8 +20,10 @@ of synthetic hidden states (the attention between MoE blocks is outside the path
           core/parallel/expert_module.cpp (oracle/_ref/ref_expert_module.so, kind "reference"; the oracle port if
           that .so is absent), at the fastest thread count of a sweep -- also used as a full-size parity check.
 --impl reference times that CPU path alone (the reference's complete native engine needs a GPU: its GPU-side
-timing is tools/ref_engine_harness.py, profiles/r02_ref_engine.json).
-N>1: expert parallel over N ranks (rank r owns experts [r*E/N, (r+1)*E/N)), weak scaling (batch 8 per rank),
+timing is tools/ref_engine_harness.py).
+--dump-outputs DIR: after the timed steps, DIR/out.npy holds the MoE block outputs of the last timed step ([layers, T, H],
+float32); the weights and inputs are drawn from fixed seeds, so two builds run with the same arguments can be compared.
+N>1: expert parallel over N ranks, all 32 layers (rank r owns experts [r*E/N, (r+1)*E/N)), weak scaling (batch 8 per rank),
 fused peer-to-peer token dispatch over NVLink (B2M_EP_EXCHANGE=nccl selects the NCCL all-to-all baseline);
 see moe_infinity_b200/ep.py.
 """
@@ -43,34 +45,60 @@ for p in (ROOT, os.path.join(ROOT, "moe-infinity_b200")):
 import torch  # noqa: E402
 
 MIXTRAL = dict(L=32, E=8, H=4096, I=14336, k=2)
+# The single-GPU all-resident headline times 16 layers: all 32 (90 GB of experts) do not fit one 80 GB H100; 16 (45 GB) are
+# the per-GPU share of Mixtral-8x7B split over two GPUs by layers.  Expert parallel (11-45 GB per rank) and forced offload
+# (HBM holds ratio x capacity) run all 32.
+RESIDENT_LAYERS_1GPU = 16
 BATCH = 8
 METRIC = "decode tokens/sec + p50 per-token latency, Mixtral-8x7B MoE dispatch path"
 
 
+# NVIDIA data-sheet peaks per H100 card (dense bf16): figures the fractions are taken against, not measured ones
+CARD_PEAKS = {
+    "sxm": dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="NVIDIA H100 SXM data sheet (HBM3 3.35 TB/s, 989 TFLOP/s bf16, at up to 700 W)"),
+    "pcie": dict(hbm_gbs=2000.0, bf16_tflops=756.0, source="NVIDIA H100 PCIe data sheet (HBM2e 2.0 TB/s, 756 TFLOP/s bf16)"),
+    "nvl": dict(hbm_gbs=3900.0, bf16_tflops=835.0, source="NVIDIA H100 NVL data sheet (HBM3 3.9 TB/s, 835 TFLOP/s bf16)"),
+}
+
+
+def card_peaks(gpu_index=0):
+    """Data-sheet peaks of the card that runs (by its reported name); an unrecognised card is taken as an H100 SXM and
+    the source string says so."""
+    name = torch.cuda.get_device_name(gpu_index) if torch.cuda.is_available() else ""
+    kind = "pcie" if "PCIe" in name else "nvl" if "NVL" in name else "sxm"
+    p = dict(CARD_PEAKS[kind])
+    if "H100" not in name:
+        p["source"] = f"card '{name}' not recognised: assumed " + p["source"]
+    return p
+
+
 def load_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            d = json.load(f)
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    """HBM bandwidth the roofline fractions are taken against, with its source."""
+    p = card_peaks()
+    return p["hbm_gbs"], p["source"]
 
 
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel (K3), from the newest COMMITTED
-    `ncu --set full` capture of this command -- a property of that capture (one layer with 7 activated experts), not of the run
-    that prints it: returned together with its source so the JSON line says so.  None if no capture is committed."""
-    for name in ("r02b_dram_traffic.json", "r01k_dram_traffic.json", "r01_k3_dram_traffic.json"):
-        path = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(path):
-            with open(path) as f:
-                d = json.load(f)
-            return d.get("traffic_bytes_per_launch"), f"profiles/{name}: {d.get('source', 'ncu --set full capture')}"
-    return None, None
+def gpu_identity(gpu_index=0):
+    """Card name and power limit: a time measured on a power-limited card is a different number."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(gpu_index), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=20).stdout
+        name, plim, smax = [x.strip() for x in out.strip().split(",")[:3]]
+        return {"name": name, "power_limit_w": float(plim), "sm_max_mhz": float(smax)}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(dirname, arrays):
+    """Write each array as DIR/<name>.npy (float32)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -214,7 +242,7 @@ def make_cpu_layer(E, H, I, dtype, seed):
 
 def cpu_sample(layer, xs, gate, experts, k, budget_s, L_model):
     """Time `n` consecutive full-size layers (fresh inputs per layer, same 2.8 GB of weights: larger than any host cache)
-    as one sample of a decode step; n = as many of the model's layers as fit the budget.  -> (sec per 32-layer step, n, reps)"""
+    as one sample of a decode step; n = as many of the model's layers as fit the budget.  -> (sec per L_model-layer step, n, reps)"""
     with torch.no_grad():
         t0 = time.perf_counter()
         layer(xs[0], gate, experts, k)
@@ -235,11 +263,12 @@ def cpu_sample(layer, xs, gate, experts, k, budget_s, L_model):
 
 def run_reference(args):
     """--impl reference: the reference's own CPU implementation of the path on the host cores.  Each step = as many of
-    the 32 full-size layers as fit the time budget (all 32 when the box is fast enough), scaled to 32; said in `config`."""
+    the full-size layers as fit the time budget (all of them when the box is fast enough), scaled to all; said in `config`."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    cfg = MIXTRAL
+    # the GPU arm's workload: 16 resident layers on one GPU, the 32-layer model under expert parallelism
+    cfg = dict(MIXTRAL, L=RESIDENT_LAYERS_1GPU if args.gpus <= 1 else MIXTRAL["L"])
     dtype = torch.bfloat16
     layer, kind = cpu_reference_layer_fn()
     experts = make_cpu_layer(cfg["E"], cfg["H"], cfg["I"], dtype, 1234)
@@ -273,7 +302,7 @@ def run_reference(args):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": step_s * 1e3, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "p50_token_latency_ms": sorted(times)[len(times) // 2] * 1e3,
-        "config": {"workload": f"Mixtral-8x7B MoE dispatch path, decode batch 8 per GPU x {max(1, args.gpus)} (T={T}), bf16, 32 layers x 8 "
+        "config": {"workload": f"Mixtral-8x7B MoE dispatch path, decode batch 8 per GPU x {max(1, args.gpus)} (T={T}), bf16, {cfg['L']} layers x 8 "
                                "experts top-2, H=4096 I=14336; the reference's CPU path (routing/combine restated from mixtral.py, expert "
                                f"FFN kind '{kind}'); {what}", "inputs": "host memory", "global_batch": T,
                    "layers": cfg["L"], "layers_timed_per_step": n_layers, "threads": threads},
@@ -306,9 +335,7 @@ def run_ours(args):
         return ep.bench_ep(args, MIXTRAL, BATCH, METRIC, load_peaks, ClockSampler)
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    cfg = dict(MIXTRAL)
-    if args.layers:
-        cfg["L"] = args.layers
+    cfg = dict(MIXTRAL, L=args.layers or RESIDENT_LAYERS_1GPU)
     L, E, H, I, k = cfg["L"], cfg["E"], cfg["H"], cfg["I"], cfg["k"]
     T = BATCH
     dtype = torch.bfloat16
@@ -343,7 +370,7 @@ def run_ours(args):
         eng.route(l, x_dev[l])
         counts.append(eng.ws("counts", T).cpu().tolist())
     bytes_step, bytes_k3_step = algorithmic_bytes(counts, T, cfg)
-    # ---- CUDA graph of one 32-layer step
+    # ---- CUDA graph of one step over all layers
     graph = torch.cuda.CUDAGraph()
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -365,6 +392,8 @@ def run_ours(args):
         evs[i + 1].record()
     torch.cuda.synchronize()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"out": out_dev})
     step_ms = [evs[i].elapsed_time(evs[i + 1]) for i in range(args.steps)]
     total_ms = evs[0].elapsed_time(evs[-1])
     ms_per_step = total_ms / args.steps
@@ -395,12 +424,11 @@ def run_ours(args):
     roofline = {"bound": "hbm", "kernel": "grouped_gemm_tc_kernel<16,dual> (gate/up + SwiGLU, K3)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "peak_source": peak_src, "avg_launch_ms": k3_avg_ms, "algorithmic_bytes_per_launch": k3_bytes,
-                "traffic": load_traffic()[0], "traffic_source": load_traffic()[1],
                 "step": {"algorithmic_bytes": bytes_step, "achieved": bytes_step / (ms_per_step * 1e-3) / 1e9,
                          "frac": bytes_step / (ms_per_step * 1e-3) / 1e9 / peak}}
 
     # ---- e2e: public API with HOST buffers -- DecodeSession.step(): pinned host -> device copy of the step's inputs,
-    # all 32 layers, device -> pinned host copy of the outputs, one stream synchronise; all inside the timed region
+    # all layers, device -> pinned host copy of the outputs, one stream synchronise; all inside the timed region
     from moe_infinity_b200 import DecodeSession
     sess = DecodeSession(eng, T).capture()
     sess.x_host.copy_(x_dev.cpu())
@@ -437,7 +465,7 @@ def run_ours(args):
     e2e = {"value": BATCH * args.steps / (e2e_ms * 1e-3), "unit": "tokens/s",
            "h2d_bytes_per_step": x_host.numel() * 2, "d2h_bytes_per_step": out_host.numel() * 2,
            "ms_per_step": e2e_ms / args.steps,
-           "api": "DecodeSession.step(): graph of H2D copy + 32 x b2m_moe_forward + D2H copy, host synchronised",
+           "api": f"DecodeSession.step(): graph of H2D copy + {L} x b2m_moe_forward + D2H copy, host synchronised",
            "eager_per_layer_api": {"value": BATCH * args.steps / (eager_ms * 1e-3), "ms_per_step": eager_ms / args.steps,
                                    "api": "MoEEngine.forward per layer (ctypes -> b2m_moe_forward)"}}
 
@@ -480,9 +508,10 @@ def run_ours(args):
                                "(outside the path)",
                    "global_batch": BATCH, "layers": L, "parallelism": "single GPU",
                    "l2": "inputs larger than L2: each step streams ~%.1f GB of distinct expert weights" % (bytes_step / 1e9),
-                   "numerics": "reference rounding chain", "timed_region": "CUDA graph replay of the 32-layer step"},
+                   "numerics": "reference rounding chain", "timed_region": f"CUDA graph replay of the {L}-layer step"},
         "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches_per_step * args.steps),
-        "launches_per_step": int(launches_per_step), "clocks": clocks, "full_size_parity_layer0": parity,
+        "launches_per_step": int(launches_per_step), "clocks": clocks, "gpu": gpu_identity(local),
+        "full_size_parity_layer0": parity,
         "setup_s": setup_s,
     }
     print(json.dumps(line), flush=True)
@@ -673,8 +702,7 @@ def run_deepseek(args):
         _view(p.value, (3 * Hh * 2 * I,), dtype, eng.device).normal_(0, 0.02)
         eng._ck(eng.lib.b2m_register_shared(eng._h, l, None, 0))
     peak, peak_src = load_peaks()
-    with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-        tf_peak = float(json.load(f).get("bf16_tflops_sustained", 1417.8))
+    tf_peak = card_peaks()["bf16_tflops"]
 
     def measure(T, iters, graph=True):
         x = torch.randn(Lr, T, Hh, device=dev).to(dtype)
@@ -762,7 +790,7 @@ def run_deepseek(args):
         "gpu_launches": int(dec["launches_per_step"] * max(args.steps, 10)), "clocks": clocks, "decode": dec,
         "prefill": None if pre is None else dict(pre, roofline={"bound": "tensor", "achieved": pre["tflops"], "peak": tf_peak,
                                                                "unit": "TFLOP/s", "frac": pre["tensor_frac"],
-                                                               "peak_source": "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"}),
+                                                               "peak_source": card_peaks()["source"]}),
     }
     print(json.dumps(line), flush=True)
 
@@ -785,7 +813,11 @@ def main():
     ap.add_argument("--layers", type=int, default=0, help="debug: fewer layers (invalid as a bench value)")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.config != "mixtral" or args.gpus != 1):
+        ap.error("--dump-outputs is implemented for the single-GPU headline run only (--config mixtral --gpus 1)")
     if args.impl == "reference":
         return run_reference(args)
     if not torch.cuda.is_available():

@@ -1,4 +1,4 @@
-/* b2m.h -- C ABI of the B200-native MoE expert dispatch/offload engine (libb2m.so).
+/* b2m.h -- C ABI of the H100-native MoE expert dispatch/offload engine (libb2m.so).
  *
  * Drop-in boundary for the ONE hot path of EfficientMoE/MoE-Infinity named in BASELINE.json:
  * router softmax/top-k -> token permute -> grouped expert GEMM -> unpermute/combine, plus the HBM expert
@@ -100,7 +100,7 @@ typedef struct b2m_config {
                                  (core/memory/memory_pool.cpp:150-158): slots = ratio * total HBM / expert bytes */
   int32_t max_inflight_prefetch; /* concurrent prefetch copies on the side stream (default 2) */
   int32_t h2d_chunk_bytes;  /* H2D copy granularity in bytes (0 = whole expert in one cudaMemcpyAsync) */
-  int32_t gemm_impl;        /* 0 = tcgen05 (product); 1 = CUDA-core cross-check kernel (bring-up only) */
+  int32_t gemm_impl;        /* 0 = wgmma tensor cores (product); 1 = CUDA-core cross-check kernel (bring-up only) */
   int32_t cache_policy;     /* B2M_CACHE_* : on-demand budget accounting */
   int32_t lookahead_prefetch; /* 1 | 2 (offload mode, T <= 256): every routing call also applies the NEXT layer's router weight
                                (b2m_set_gate) to this layer's input and reads the predicted expert counts back with this

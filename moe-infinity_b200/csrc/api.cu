@@ -39,32 +39,29 @@ constexpr int STAGE_RING = 8;
 
 std::string g_create_error;
 
-// ---- run-time switches: read ONCE per process, here and nowhere else in this file.  Every default is the setting that
-// measured best on a B200 (DESIGN.md §6 has the A/B numbers); the others stay selectable for re-measurement.
+// ---- run-time switches: read ONCE per process, here and nowhere else in this file.  The alternative to every default
+// stays selectable for A/B measurement (DESIGN.md §6).
 struct Switches {
-  bool nt256, nt256_up, pdl, early_k3, rows_by_gate, pdl_k3, dyn_n, early_a, streamk, ep_early_combine, ep_direct, ep_mrows, timeline, fused_ffn;
+  bool nt256, pdl, early_k3, rows_by_gate, pdl_k3, early_a, streamk, ep_early_combine, ep_direct, ep_mrows, timeline, fused_ffn;
   int ep_l2pf_mb;
   long long nt256_min_avg;
   static bool off(const char* n) { const char* v = getenv(n); return v && v[0] == '0'; }   // default on
   static bool on(const char* n) { const char* v = getenv(n); return v && v[0] == '1'; }    // default off
   Switches()
-      : nt256(!off("B2M_NT256")),                 // 256-token tiles in the tensor-bound regime
-        nt256_up(!off("B2M_NT256_UP")),           // ... for the gate/up GEMM too (B2M_NUMERICS_FP32 only)
-        pdl(on("B2M_PDL")),                       // programmatic dependent launch on every decode kernel: 2.5 % slower
+      : nt256(!off("B2M_NT256")),                 // 256-token tiles for the down projection in the tensor-bound regime
+        pdl(on("B2M_PDL")),                       // programmatic dependent launch on every decode kernel
         early_k3(!off("B2M_EARLY_K3")),           // gate/up GEMM prefetches weights under the permute kernel
         rows_by_gate(!off("B2M_ROWS_BY_GATE")),   // the last gate/top-k CTA publishes the row maps
         pdl_k3(on("B2M_PDL_K3")),
-        dyn_n(on("B2M_DYN_N")),                   // per-tile MMA width: +1.5 % at DeepSeek prefill (profiles/r02a_deepseek_dyn_n.json), parity untested -> off
         early_a(!off("B2M_EARLY_A")),             // down GEMM prefetches weights under the gate/up GEMM's tail
         streamk(!off("B2M_STREAMK")),             // stream-K partition of the split-K down GEMM
         ep_early_combine(!off("B2M_EP_EARLY_COMBINE")),
         ep_mrows(!off("B2M_EP_MROWS")),
-        ep_l2pf_mb(getenv("B2M_EP_L2PF_MB") ? atoi(getenv("B2M_EP_L2PF_MB")) : 0),   // L2 prefetch of gate/up weights behind programmatic edges: N=2 7.94 vs 7.93, N=4 4.78 vs 4.79 ms/step -> opt-in
+        ep_l2pf_mb(getenv("B2M_EP_L2PF_MB") ? atoi(getenv("B2M_EP_L2PF_MB")) : 0),   // L2 prefetch of gate/up weights behind programmatic edges: opt-in
         ep_direct(!off("B2M_EP_DIRECT")),         // four-launch expert-parallel layer
         timeline(on("B2M_TIMELINE")),             // device timestamps of the expert-parallel layer (diagnostics)
-        fused_ffn(on("B2M_FUSED_FFN")),           // (only in -DB2M_ENABLE_FUSED_FFN builds) gate/up + down GEMMs in one persistent kernel: measured
-                                                  // 12.89 vs 12.84 ms/step (Mixtral) and 5.04 vs 4.75 ms (DeepSeek: it keeps the
-                                                  // side-stream shared-expert GEMMs off the SMs) -> opt-in
+        fused_ffn(on("B2M_FUSED_FFN")),           // (only in -DB2M_ENABLE_FUSED_FFN builds) gate/up + down GEMMs in one persistent kernel
+                                                  // (it keeps the side-stream shared-expert GEMMs off the SMs) -> opt-in
         nt256_min_avg(getenv("B2M_NT256_MIN_AVG") ? atoll(getenv("B2M_NT256_MIN_AVG")) : 256) {}
 };
 const Switches& sw() {
@@ -119,7 +116,7 @@ struct Slot {
 struct b2m_ctx {
   b2m_config cfg;
   std::string err;
-  int num_sms = 148;
+  int num_sms = 132;
   size_t total_mem = 0;
   PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
 
@@ -338,12 +335,10 @@ int pick_nt(int T) {
   return 128;
 }
 // tensor-bound regime: 256-token tiles when the average expert sees at least one full tile
-// (B2M_NT256=0 disables).  Measured (profiles/r01f_prefill.txt): down 3.40 -> 2.65 ms (1.45 PFLOP/s, tensor pipe 92 %).
-// The gate/up GEMM's two 256-column accumulators leave no second TMEM stage, so its SwiGLU epilogue serialises with the
-// MMAs: with the precise expf/div epilogue it got slower (7.2 -> 8.1 ms), with the MUFU epilogue faster (-> 6.6 ms).
+// (B2M_NT256=0 disables): a weight tile read once serves twice the tokens.  Down projection only (see plan_gemm).
 int pick_nt_model(const b2m_config& f, int T) {
   const long long avg = (long long)T * f.top_k / f.num_experts;
-  if (sw().nt256 && avg >= sw().nt256_min_avg && f.hidden >= 256) return 256;   // DeepSeek-V2-Lite prefill (avg 384): 27.6 -> 25.1 ms
+  if (sw().nt256 && avg >= sw().nt256_min_avg && f.hidden >= 256) return 256;
   return pick_nt(T);
 }
 
@@ -627,12 +622,9 @@ RouteParams base_route_params(b2m_ctx* c, int layer, const void* x, int T, int s
 void plan_gemm(b2m_ctx* c, int T) {
   c->cur_T = T;
   c->cur_nt_dn = pick_nt_model(c->cfg, T);
-  // gate/up GEMM: 256-token tiles too (single TMEM stage, MUFU SiLU epilogue): 7.37 -> 6.61 ms at T=16384
-  // (profiles/r01f_prefill.txt); B2M_NT256_UP=0 keeps the 128-token double-buffered tiles
-  const bool up256 = sw().nt256_up;
-  // reference numerics keep the precise SiLU, with which the single-stage 256-token tile is slower than the double-buffered
-  // 128-token tile (8.1 vs 7.2-7.4 ms): 256 for the gate/up GEMM only in B2M_NUMERICS_FP32 mode
-  c->cur_nt = (up256 && c->cur_nt_dn == 256 && c->cfg.numerics == B2M_NUMERICS_FP32) ? 256 : pick_nt(T);
+  // gate/up GEMM: at most 128-token tiles -- its two accumulators (gate and up) of a 256-token tile would need 256 fp32
+  // registers per thread of a wgmma warpgroup
+  c->cur_nt = pick_nt(T);
   c->cur_ksplit = pick_ksplit(c, T, c->cfg.hidden, c->cfg.inter, c->cfg.num_experts, c->cfg.top_k, c->cur_nt_dn);
   if (c->arena.shape.has_bias) c->cur_ksplit = 1;   // `+ fc2_bias` is applied once, in the epilogue of the whole-K product
   if (c->cfg.dtype == B2M_DTYPE_F32) c->cur_ksplit = 1;   // CUDA-core fp32 path: whole-K tiles
@@ -698,8 +690,8 @@ int b2m_ctx_create(const b2m_config* cfg, b2m_ctx** out) {
   CKC(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CKC(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) {
-    fail(nullptr, B2M_EUNSUPPORTED, "device sm_%d%d: this library is built for sm_100a (B200) only", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    fail(nullptr, B2M_EUNSUPPORTED, "device sm_%d%d: this library is built for sm_90a (H100) only", prop.major, prop.minor);
     b2m_ctx_destroy(c);
     return B2M_EUNSUPPORTED;
   }
@@ -1117,9 +1109,9 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
     if (phases & 2)
       CK(c, launch_grouped_gemm_simt(f.dtype, a.base, slot_elems, s.off_down / 2, s.off_down / 2, b_down, s.I, dn, false, st));
   } else {
-    // tensor-bound regime (several 128-token tiles per expert): a 2-CTA cluster variant that multicasts the weight tiles was
-    // measured to give no gain on B200 (L2 already de-duplicates the two CTAs' requests; the SM ingest port is the limit):
-    // compiled only with -DB2M_ENABLE_MC2 (then selected with B2M_MC2=1), not part of the default library
+    // tensor-bound regime (several 128-token tiles per expert): a 2-CTA cluster variant that multicasts the weight tiles is
+    // compiled only with -DB2M_ENABLE_MC2 (then selected with B2M_MC2=1), not part of the default library (L2 already
+    // de-duplicates the two CTAs' requests)
 #ifdef B2M_ENABLE_MC2
     static const bool mc2_on = getenv("B2M_MC2") && getenv("B2M_MC2")[0] == '1';
     const bool mc2 = mc2_on && nt == 128 && T_hint_large;
@@ -1127,9 +1119,6 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
     const bool mc2 = false;
 #endif
     const bool pdl_k3 = sw().pdl_k3;
-    // experimental, default off and not yet measured: per-tile MMA width (ragged last token tiles of prefill-sized experts)
-    const bool dyn_n = sw().dyn_n;
-    up.dyn_n = dn.dyn_n = (dyn_n && T_hint_large && !mc2) ? 1 : 0;
     up.pdl_edge = (pdl_k3 && !T_hint_large) ? 1 : 0;
     up.early_a = (c->k3_early_ok && &a == &c->arena && phases == 3) ? 1 : 0;   // routed experts right behind the permute kernel
     // decode regime, routed experts, both phases in one call: ONE persistent kernel (gate/up phase, grid barrier, down phase)
@@ -1155,11 +1144,12 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
     }
     if (phases & 2) {
       // prefill-sized token tiles: pair two m-tiles of the down matrix on one token tile (dual_m) -> 1.33x the
-      // FLOP per operand byte; decode keeps single tiles (finer split-K balance, HBM bound anyway)
-      const bool pair = nt_dn >= 128 && s.H >= 256 && T_hint_large;
+      // FLOP per operand byte; decode keeps single tiles (finer split-K balance, HBM bound anyway).  256-token tiles already
+      // share each weight tile between twice the tokens, and a paired 256-token tile has no room in the registers.
+      const bool pair = nt_dn == 128 && s.H >= 256 && T_hint_large;
       dn.dual_m = pair ? 1 : 0;
       // decode: let the down projection start under the tail of the gate/up GEMM and prefetch its first weight tiles
-      // measured on B200 (profiles/r01g_pdl_edges.txt): 12.945 -> 12.855 ms/step; B2M_EARLY_A=0 disables
+      // B2M_EARLY_A=0 disables
       const bool early_a = sw().early_a;
       dn.early_a = (early_a && !pdl_enabled() && (phases & 1) && f.gemm_impl == 0 && !T_hint_large) ? 1 : 0;
       // split-K at decode: equal contiguous shares of all (tile, k-block) units per CTA instead of a fixed factor, so no
@@ -1330,9 +1320,9 @@ int b2m_run_experts_ex(b2m_ctx* c, int layer, int T, int phases, void* stream) {
                     remaining.end());
   }
   c->last_active = wave;   // experts of the last wave are still being read by kernels in flight
-  // Measured on a B200 (profiles/r02_offload_config3.json): when the host->device link is saturated by on-demand copies a
-  // prefetch cannot save time, only bytes -- and a wrong prediction costs a whole expert (6.4 ms for Mixtral): with ~80 %
-  // accurate predictions unconditional prefetching LOST 12 % against the same cache without it.  So (lookahead_prefetch = 1)
+  // When the host->device link is saturated by on-demand copies a prefetch cannot save time, only bytes -- and a wrong
+  // prediction costs a whole expert (352 MB for Mixtral), so ~80 % accurate predictions lose against the same cache
+  // without prefetching.  So (lookahead_prefetch = 1)
   // predictions are staged only from layers that staged nothing on demand, i.e. into link time that is otherwise idle;
   // lookahead_prefetch = 2 prefetches unconditionally (sparse-miss regimes, ablations).
   if (c->cfg.lookahead_prefetch == 1 && c->pf_win_useful + c->pf_win_wasted >= 16) {
@@ -1914,12 +1904,11 @@ int b2m_ep_p2p_layer(b2m_ctx* c, int layer, const void* x, const void* router_in
   }
   const int ni = nt_index(nt);
   if (tl) { up.tl = tl + 4; dn.tl = tl + 8; }
-  // The tile list is static here, so the grid can be sized to it: with 448 tiles (4 experts x 112) on 148 CTAs the last 4
-  // tiles run alone and are limited by what one SM can ingest (~120 GB/s; measured 17 us of a 162 us kernel,
-  // profiles/r02_ep2_timeline_before.log); 112 CTAs x 4 tiles each finish together at the full HBM rate.
-  // Weight rows per tile: 128-row tiles cut I = 14336 into 112 tiles per expert, which leaves 36 of 148 SMs idle when a rank
-  // owns one expert (N = 8) and a 128-row tile is bound by what one SM ingests (profiles/r02_ep8_timeline.log).  Tiles of
-  // m_rows = roundup8(El*I / (SMs * rounds)) rows (104 -> 138 tiles per expert) put every SM to work; the MMA stays M = 128.
+  // The tile list is static here, so the grid can be sized to it: with 448 tiles (4 experts x 112) on 132 CTAs the last
+  // tiles of an uneven last round run alone, limited by what one SM can ingest; 112 CTAs x 4 tiles each finish together.
+  // Weight rows per tile: 128-row tiles cut I = 14336 into 112 tiles per expert, which leaves 20 of 132 SMs idle when a rank
+  // owns one expert (N = 8) and a 128-row tile is bound by what one SM ingests.  Tiles of
+  // m_rows = roundup8(El*I / (SMs * rounds)) rows (112 -> 128 tiles per expert) put every SM to work; the MMA stays M = 128.
   if (!q.m_rows) {
     q.m_rows = 128;
     if (sw().ep_mrows && s.dual) {

@@ -44,8 +44,6 @@ struct GemmParams {
   int pdl_edge;         // launch with a programmatic edge (prologue overlaps the predecessor's tail; waits before any global access)
   int early_a;          // launched with a programmatic edge: weight tiles may be fetched before the predecessor finishes
   int dual_m;           // DUAL kernel, EPI_LINEAR_F32: A1 = rows m0+128.. of the same matrix (two m-tiles share a token tile)
-  int dyn_n;            // experimental (B2M_DYN_N=1, default off, unmeasured): issue each tile's MMAs with N = its token count
-                        // rounded up to 16 instead of the full tile width, so ragged last token tiles cost proportionally less
   // bias experts (NLLB / FSGPT, expert_module.cpp:88-92,124-128): bias[m] of the expert in slot s lives at
   // bias_base + s * bias_slot_elems + bias_off (16-bit elements of the model dtype); null = no bias.  Needs ksplit == 1.
   const void* bias_base;

@@ -188,7 +188,7 @@ static bool ep_ok(const EpParams& p) {
   return p.nranks >= 1 && p.nranks <= EP_MAX_RANKS && p.E % p.nranks == 0 && p.E / p.nranks <= EP_MAX_EL &&
          p.rank >= 0 && p.rank < p.nranks && p.cap >= 1 && p.H % 8 == 0 && (!p.inline_counts || p.E * 4 <= p.H * 2);
 }
-static int ep_grid(int rows) { return rows < 1 ? 1 : (rows > 148 * 4 ? 148 * 4 : rows); }
+static int ep_grid(int rows) { return rows < 1 ? 1 : (rows > H100_SMS * 4 ? H100_SMS * 4 : rows); }
 
 cudaError_t launch_ep_pack(const EpParams& p, int max_rows, cudaStream_t st) {
   if (!ep_ok(p)) return cudaErrorInvalidValue;

@@ -10,8 +10,7 @@ __device__ __forceinline__ void st_release_sys(int* p, int v) {
 }
 // Flag store of a release SEQUENCE: the caller has issued one __threadfence_system() after its last payload store; the flag
 // stores to the N peers are then relaxed, so they leave back to back.  (N st.release.sys in a row cost N NVLink round trips:
-// each one is a system fence that waits for the previous peer's flag store to be acknowledged -- measured ~20 us of a 129 us
-// layer at N = 8, profiles/r02e_ep8_timeline.json.)
+// each one is a system fence that waits for the previous peer's flag store to be acknowledged.)
 __device__ __forceinline__ void st_relaxed_sys(int* p, int v) {
   asm volatile("st.relaxed.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }

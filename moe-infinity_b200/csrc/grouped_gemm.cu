@@ -1,4 +1,4 @@
-// grouped_gemm.cu -- K3/K4: grouped (per-expert segmented) expert GEMMs on tcgen05 tensor cores.
+// grouped_gemm.cu -- K3/K4: grouped (per-expert segmented) expert GEMMs on Hopper wgmma tensor cores.
 //
 // Replaces the per-expert ATen loop of the reference, core/parallel/expert_module.cpp:171-175 (Mixtral),
 // :200-203 (DeepSeek), :31-35 (Switch): `matmul(act(matmul(x, w1^T)) * matmul(x, w3^T), w2^T)` issued as
@@ -6,11 +6,13 @@
 // (core/parallel/expert_dispatcher.cpp:309-395).
 //
 // Design (decode-first, "swap-AB"): the expert weight matrix [M rows, K] (nn.Linear layout, K-major) is the
-// UMMA *A* operand (M = 128 rows per tile, streamed once from HBM by TMA), the expert's tokens
-// [n_e, K] are the UMMA *B* operand (N = NT in {16,32,64,128} tokens).  D[128, NT] accumulates in TMEM.
+// wgmma *A* operand (128 rows per tile = two m64 halves, streamed once from HBM by TMA), the expert's tokens
+// [n_e, K] are the *B* operand (N = NT in {16,32,64,128,256} tokens).  D[128, NT] accumulates in registers.
 // One persistent CTA per SM walks a device-side tile list derived from the per-expert token offsets the
-// routing kernel produced -- no host sync.  Warp roles: w0 TMA producer, w1 MMA issuer (one lane),
-// w2 TMEM allocator, w4..7 epilogue (tcgen05.ld -> activation -> global).
+// routing kernel produced -- no host sync.  Roles: warpgroup 0 = TMA producer (one lane); consumer warpgroups
+// 1 and 2 each own one 64-row half of the tile (all NT columns): they issue its wgmmas out of the shared-memory ring and
+// run the epilogue (activation -> global) from their registers while the producer already fills the ring for the
+// next tile.
 //   DUAL  = gate and up projections share the token tile and are fused with act(g)*u in the epilogue.
 //   !DUAL = single projection: activation epilogue (Switch wi + ReLU) or linear fp32 output
 //           (down projection), optionally split-K with fp32 red.add.
@@ -21,16 +23,12 @@
 
 namespace b2m {
 
-constexpr int BLOCK_M = 128;   // weight rows per tile  (UMMA M)
+constexpr int BLOCK_M = 128;   // weight rows per tile
 constexpr int BLOCK_K = 64;    // 64 x 16-bit = 128 B = one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
-constexpr int GEMM_THREADS = 256;
 constexpr int MAX_E = 256;
-constexpr int SMEM_BUDGET = 216 * 1024;
-#ifndef B2M_EPI_WARPS_256
-#define B2M_EPI_WARPS_256 16   // epilogue warps of the 256-token-tile instantiations (4 per TMEM lane quadrant; measured 8: 6.6 ms, 16: 5.5-6.0 ms, 24: same)
-#endif
+constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on sm_90; the rest holds barriers and tile tables
 
 template <int NT, bool DUAL>
 struct GemmCfg {
@@ -38,20 +36,26 @@ struct GemmCfg {
   static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_TILE_BYTES + B_TILE_BYTES;
   static constexpr int STAGES_RAW = SMEM_BUDGET / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 10 ? 10 : STAGES_RAW;
-  static constexpr int ACC_COLS = (DUAL ? 2 : 1) * NT;
-  // NT=256 with two accumulators fills the 512 TMEM columns with ONE stage (no MMA/epilogue overlap); it is used in the
-  // tensor-bound regime because it halves the weight bytes an SM has to ingest per FLOP (the SM ingest port, ~64 B/clk,
-  // is what limited the 128-token tiles to ~65 % tensor-pipe activity).  Eight epilogue warps shorten the bubble.
-  static constexpr int ACC_STAGES = (ACC_COLS * 2 <= 512) ? 2 : 1;
-  static constexpr int EPI_WARPS = (NT >= 256) ? B2M_EPI_WARPS_256 : 4;
-  static constexpr int THREADS = 128 + 32 * EPI_WARPS;
-  static constexpr int TMEM_COLS_RAW = ACC_COLS * ACC_STAGES;
-  static constexpr int TMEM_COLS = TMEM_COLS_RAW <= 32 ? 32 : TMEM_COLS_RAW <= 64 ? 64 : TMEM_COLS_RAW <= 128 ? 128
-                                   : TMEM_COLS_RAW <= 256 ? 256 : 512;
+  // a consumer warpgroup holds a 64 x NT fp32 accumulator (NT/2 registers per thread, twice for DUAL): a DUAL 256-token
+  // tile (256 accumulator registers per thread) does not exist
+  static constexpr int ACC_REGS = NT / 2;
+  static constexpr int CONSUMERS = 2;     // warpgroups: one per 64-row half of the tile
+  static constexpr int THREADS = 128 * (1 + CONSUMERS);
+  // setmaxnreg split of the CTA's registers: the block is launched with LAUNCH_REGS per thread (what __launch_bounds__ leaves
+  // for one block of THREADS per SM, rounded down to the allocation granule of 8); setmaxnreg only moves registers inside
+  // that allocation, so the producer warpgroup (one issuing lane) drops to 40 and the consumers take what it frees (a
+  // request beyond the allocation would never be granted).  launch_tc checks LAUNCH_REGS against the compiled kernel.
+  static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
+  static constexpr int PRODUCER_REGS = 40;
+  static constexpr int CONSUMER_REGS_RAW = (LAUNCH_REGS * THREADS - 128 * PRODUCER_REGS) / (128 * CONSUMERS);
+  static constexpr int CONSUMER_REGS = (CONSUMER_REGS_RAW > 240 ? 240 : CONSUMER_REGS_RAW) & ~7;
+  static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 128 * CONSUMERS <= LAUNCH_REGS * THREADS, "register split too large");
+  static_assert(CONSUMER_REGS >= LAUNCH_REGS, "setmaxnreg.inc must not lower the consumers' count");
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ +
                                     (MAX_E + 1) * 4 * 2 /*tile_start, offsets*/ + MAX_E * 4 * 2 /*slots, region counts*/;
-  static_assert(TMEM_COLS_RAW <= 512, "TMEM overflow");
+  static_assert(!(DUAL && NT > 128), "DUAL tiles are at most 128 tokens wide");
   static_assert(STAGES >= 2, "need >=2 stages");
+  static_assert(SMEM_BYTES <= 227 * 1024, "over the sm_90 shared-memory limit");
 };
 
 __device__ __forceinline__ float act_apply(float x, int act) {
@@ -61,15 +65,19 @@ __device__ __forceinline__ float act_apply(float x, int act) {
   return x;
 }
 
-// SiLU with the MUFU approximations (ex2.approx, rcp.approx).  Used only by the 256-token-tile instantiation in
-// B2M_NUMERICS_FP32 mode (its single TMEM stage makes the epilogue serialise with the MMAs; the epilogue gets ~3x shorter).
-// B2M_NUMERICS_REFERENCE always uses the precise form: the ~2 ulp(fp32) of the approximations would survive the following
-// round-to-model-dtype in ~1e-3 of the elements.
-__device__ __forceinline__ float silu_mufu(float x) {
-  float e, r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-x * 1.4426950408889634f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-  return x * r;
+// the four k16 steps of one 64-wide k-block for a 64 x W accumulator
+template <int W, int DT>
+__device__ __forceinline__ void wgmma_kblock(float (&d)[W / 2], uint64_t da, uint64_t db, bool first) {
+#pragma unroll
+  for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+    const uint64_t koff = (uint64_t)((k * MMA_K * 2) >> 4);   // advance the start address inside the SW128 atom
+    const uint32_t acc = (!first || k > 0) ? 1u : 0u;
+    if constexpr (W == 16) wgmma_m64n16k16<DT>(d, da + koff, db + koff, acc);
+    else if constexpr (W == 32) wgmma_m64n32k16<DT>(d, da + koff, db + koff, acc);
+    else if constexpr (W == 64) wgmma_m64n64k16<DT>(d, da + koff, db + koff, acc);
+    else if constexpr (W == 128) wgmma_m64n128k16<DT>(d, da + koff, db + koff, acc);
+    else wgmma_m64n256k16<DT>(d, da + koff, db + koff, acc);
+  }
 }
 
 // expert-parallel direct mode: wait (one thread) until every source rank has published this layer's epoch, i.e. its rows
@@ -97,23 +105,20 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
   } while (v == g.gen);
 }
 
-// One grouped GEMM over the device-side tile list: TMA producer / MMA issuer / epilogue warps over a shared-memory ring.
+// One grouped GEMM over the device-side tile list: a TMA producer and the wgmma consumer warpgroups over a shared-memory ring.
 // Used as the whole body of grouped_gemm_tc_kernel and, twice, by fused_ffn_kernel (gate/up phase, grid barrier, down phase).
-// TMEM is allocated by the caller (tmem_base); `ctas` = how many CTAs of the grid take tiles of this phase.
-template <int NT, bool DUAL, int DT, int MC>
+// `ctas` = how many CTAs of the grid take tiles of this phase.  REGSPLIT: rebalance registers between producer and consumers
+// (once per kernel: the two-phase fused kernel keeps the even split).
+template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
-                                          const GemmParams& p, uint8_t* smem, uint32_t tmem_base, int dep_mode,
-                                          const GridBar& gbar, int ctas) {
+                                          const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
   using Cfg = GemmCfg<NT, DUAL>;
-  // carve shared memory: [stages | barriers | tmem ptr | tile tables]
+  // carve shared memory: [stages | barriers | tile tables]
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = tmem_full + Cfg::ACC_STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + Cfg::ACC_STAGES);
-  int* tile_start = reinterpret_cast<int*>(tmem_ptr_smem + 2);
+  int* tile_start = reinterpret_cast<int*>(empty_bar + Cfg::STAGES);
   int* offs = tile_start + (MAX_E + 1);
   int* slots = offs + (MAX_E + 1);
   int* cnts = slots + MAX_E;           // direct mode: rows per expert region
@@ -125,8 +130,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   // dual_m: the two A tiles are rows [m0, m0+128) and [m0+128, m0+256) of the SAME matrix sharing one token tile
   // (doubles the arithmetic intensity of the down projection at prefill; the kernel is L2->SM operand-bandwidth bound)
   // m_rows (EP region mode, MC == 1): weight rows a tile really covers (a multiple of 8, <= 128; the A tensor maps carry a box of
-  // that many rows).  The MMA still runs M = 128; the tail rows of the stage hold stale bytes and their accumulator lanes are
-  // dropped in the epilogue.  Lets the host cut I rows into as many tiles as there are SMs (14336 / 104 = 138 <= 148).
+  // that many rows).  The MMA still runs M = 128; the tail rows of the stage hold stale bytes and their accumulator rows are
+  // dropped in the epilogue.  Lets the host cut I rows into as many tiles as there are SMs (14336 / 112 = 128 <= 132).
   const int m_rows = (MC == 1 && !p.dual_m && p.m_rows > 0) ? p.m_rows : BLOCK_M;
   const int m_step = (DUAL && p.dual_m) ? 2 * BLOCK_M : m_rows;
   const int m_tiles = (p.M + m_step - 1) / m_step;
@@ -140,16 +145,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], MC);   // with multicast operands a stage is free when every CTA of the cluster consumed it
-    }
-    for (int a = 0; a < Cfg::ACC_STAGES; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], Cfg::EPI_WARPS);
+      // a stage is free when every consumer warpgroup -- with multicast operands: of every CTA of the cluster -- consumed it
+      mbar_init(&empty_bar[s], Cfg::CONSUMERS * MC);
     }
     fence_barrier_init();
   }
   // Expert parallel (direct mode): this kernel's CTAs are resident while the routing kernel is still exchanging rows with the peers
-  // and the previous layer's combine waits for its owners -- HBM is idle for ~30 us per layer (profiles/r02e_ep8_timeline.json).
+  // and the previous layer's combine waits for its owners, so HBM idles at the start of every layer.
   // Each CTA asks the TMA unit to pull the first ep_l2pf k-blocks of the weight tiles it will most likely own (one token tile
   // per local expert: tile = le * m_tiles + m) into L2.  A hint only: a wrong guess costs bandwidth, never correctness.  The slot
   // table is older than any predecessor in the stream.
@@ -205,9 +207,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
     }
     tile_start[E] = acc;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   const int crank = MC > 1 ? (int)cluster_ctarank() : 0;
   if (MC > 1) cluster_sync_all();   // peers' barriers are initialised before any multicast targets them
 
@@ -224,9 +224,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   const int tile_stride = ctas / MC;
   const int tile0 = (int)blockIdx.x < ctas ? (int)blockIdx.x / MC : 0x3fffffff;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    if constexpr (REGSPLIT) setmaxnreg_dec<Cfg::PRODUCER_REGS>();
     // ===================== TMA producer (one lane) =====================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       bool waited = !p.early_a;
@@ -247,7 +248,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
           } else {
             // 2-CTA multicast: the cluster's CTAs work on the same weight tiles and adjacent token tiles; each CTA fetches
             // HALF of every weight tile (64 rows; tmA* carry 64-row boxes) and multicasts it into both CTAs' stages, so
-            // a CTA pulls 16+16 KB instead of 32+16 KB per k-block from L2 (the kernel is L2->SM operand-bandwidth bound)
+            // a CTA pulls 16+16 KB instead of 32+16 KB per k-block from L2
             const int half = crank * (BLOCK_M / 2);          // rows this CTA fetches
             const int hoff = crank * (A_TILE_BYTES / 2);     // where they sit inside the 128-row stage tile
             tma_load_3d_mc(&tmA0, &full_bar[stage], sA0 + hoff, kb * BLOCK_K, t.m0 + half, t.slot, (uint16_t)0x3, wh);
@@ -279,147 +280,123 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
                       pend_kb[i] * BLOCK_K, pend_row[i], CACHE_EVICT_LAST);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one lane) =====================
+  } else {
+    if constexpr (REGSPLIT) setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+    // ===================== consumer warpgroups: wgmma + epilogue =====================
     if (p.early_a && dep_mode == DEP_PDL) pdl_wait();
-    constexpr uint32_t idesc = make_idesc_f16(DT, BLOCK_M, NT);
+    const int ct = threadIdx.x - 128;    // thread index among all consumers
+    if (p.ep_rows > 0 && p.ep_zero) {
+      // clear the down projection's accumulator: safe now -- a source rank publishes this layer's flag only after its
+      // combine of the previous layer has finished reading the previous outputs
+      float4* z = reinterpret_cast<float4*>(p.ep_zero);
+      const size_t n4 = p.ep_zero_elems / 4;
+      const int et = Cfg::CONSUMERS * 128;
+      for (size_t i = (size_t)blockIdx.x * et + ct; i < n4; i += (size_t)gridDim.x * et)
+        z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    const int mh = ct >> 7;                  // consumer warpgroup = row half of the tile
+    const bool signaller = (ct & 127) == 0;  // releases ring stages for its warpgroup
+    const int ra = mh * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2);   // tile rows of this thread: ra, ra + 8
+    const int cb = (lane & 3) * 2;                                   // token columns: cb + 8j + {0, 1}
+    float acc0[Cfg::ACC_REGS];
+    float acc1[DUAL ? Cfg::ACC_REGS : 1];
     int stage = 0;
     uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    auto release = [&](int s) {
+      if (!signaller) return;
+      if (MC == 1) mbar_arrive(&empty_bar[s]);
+      else for (int c = 0; c < MC; ++c) mbar_arrive_cluster(&empty_bar[s], (uint32_t)c);   // the peer multicasts into it too
+    };
     for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d0 = tmem_base + acc * Cfg::ACC_COLS;
-      uint32_t idesc_t = idesc;
-      if (p.dyn_n) {   // opt-in: N of this tile's MMAs = its own token count (multiple of 16, >= 16)
-        const int n_eff = t.ncols <= 16 ? 16 : ((t.ncols + 15) & ~15);
-        idesc_t = make_idesc_f16(DT, BLOCK_M, n_eff < NT ? n_eff : NT);
-      }
+      int prev = -1;
       for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a0 = smem_u32(stage_base + stage * Cfg::STAGE_BYTES);
-          const uint32_t a1 = a0 + A_TILE_BYTES;
-          const uint32_t b = a0 + (DUAL ? 2 : 1) * A_TILE_BYTES;
-          const uint64_t da0 = make_kmajor_sw128_desc(a0);
-          const uint64_t da1 = make_kmajor_sw128_desc(a1);
-          const uint64_t db = make_kmajor_sw128_desc(b);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint32_t accum = (kb > t.kb_begin || k > 0) ? 1u : 0u;
-            const uint64_t koff = (uint64_t)((k * UMMA_K * 2) >> 4);  // advance start address inside the SW128 atom
-            tc_mma_f16(d0, da0 + koff, db + koff, idesc_t, accum);
-            if (DUAL) tc_mma_f16(d0 + NT, da1 + koff, db + koff, idesc_t, accum);
-          }
-          if (MC == 1) tc_commit(&empty_bar[stage]);  // frees the smem stage when these MMAs retire
-          else tc_commit_mc(&empty_bar[stage], (uint16_t)0x3);   // ... in both CTAs: the peer multicasts into it too
-        }
-        __syncwarp();
+        const uint32_t a0 = smem_u32(stage_base + stage * Cfg::STAGE_BYTES) + mh * (64 * BLOCK_K * 2);
+        const uint32_t b = smem_u32(stage_base + stage * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_TILE_BYTES);
+        wgmma_fence_regs(acc0);
+        if (DUAL) wgmma_fence_regs(acc1);
+        wgmma_fence();
+        wgmma_kblock<NT, DT>(acc0, make_kmajor_sw128_desc(a0), make_kmajor_sw128_desc(b), kb == t.kb_begin);
+        if constexpr (DUAL) wgmma_kblock<NT, DT>(acc1, make_kmajor_sw128_desc(a0 + A_TILE_BYTES), make_kmajor_sw128_desc(b), kb == t.kb_begin);
+        wgmma_commit();
+        wgmma_fence_regs(acc0);
+        if (DUAL) wgmma_fence_regs(acc1);
+        wgmma_wait<1>();                 // the previous k-block's wgmmas have read their operands: that stage may be refilled
+        if (prev >= 0) release(prev);
+        prev = stage;
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
       }
-      if (lane == 0) tc_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-      __syncwarp();
-      if (++acc == Cfg::ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (4 warps = 128 TMEM lanes) =====================
-    if (p.early_a && dep_mode == DEP_PDL) pdl_wait();
-    if (p.ep_rows > 0) {
-      if (p.ep_zero) {
-        // clear the down projection's accumulator: safe now -- a source rank publishes this layer's flag only after its
-        // combine of the previous layer has finished reading the previous outputs
-        float4* z = reinterpret_cast<float4*>(p.ep_zero);
-        const size_t n4 = p.ep_zero_elems / 4;
-        const int et = Cfg::EPI_WARPS * 32;
-        for (size_t i = (size_t)blockIdx.x * et + (threadIdx.x - 128); i < n4; i += (size_t)gridDim.x * et)
-          z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-    const int q = warp & 3;              // TMEM lane quadrant this warp may access
-    const int cgrp = (warp - 4) >> 2;    // with 8 epilogue warps two warps share a quadrant and alternate 16-column chunks
-    const int r = q * 32 + lane;         // weight row inside the tile
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * Cfg::ACC_COLS;
-      const int m = t.m0 + r;
-      const bool row_ok = m < p.M && r < m_rows;
-      float bias0 = 0.f, bias1 = 0.f;   // bias experts: one value per weight row = per TMEM lane
-      if (p.bias_base) {
-        const uint16_t* bp = reinterpret_cast<const uint16_t*>(p.bias_base) + (size_t)t.slot * p.bias_slot_elems + p.bias_off;
-        if (row_ok) bias0 = Half16<DT>::to_f(bp[m]);
-        if (DUAL && m + BLOCK_M < p.M) bias1 = Half16<DT>::to_f(bp[m + BLOCK_M]);
-      }
-      for (int c0 = cgrp * 16; c0 < t.ncols; c0 += 16 * (Cfg::EPI_WARPS / 4)) {   // warp-uniform trip count
-        uint32_t vg[16], vu[16];
-        tmem_ld_x16(taddr + c0, vg);
-        if (DUAL) tmem_ld_x16(taddr + NT + c0, vu);
-        tmem_ld_wait();
-        if (p.epi == EPI_LINEAR_F32) {
-          float* out = reinterpret_cast<float*>(p.out);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc0);
+      if (DUAL) wgmma_fence_regs(acc1);
+      if (prev >= 0) release(prev);
+
+      float bias0[2] = {0.f, 0.f}, bias1[2] = {0.f, 0.f};   // bias experts: one value per weight row
+      bool row_ok[2], row2_ok[2];
+      int mrow[2];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (c0 + j < t.ncols) {
-              float* dst = out + (size_t)(t.row0 + c0 + j) * p.ld_out + m;
-              if (row_ok) {
-                float v = __uint_as_float(vg[j]);
-                if (p.bias_base) v = p.mimic ? round_dt<DT>(round_dt<DT>(v) + bias0) : v + bias0;   // matmul, then `+ bias`
-                if (p.ksplit > 1) atomicAdd(dst, v); else *dst = v;
-              }
-              if (DUAL && m + BLOCK_M < p.M) {   // dual_m: second accumulator = rows m0+128..m0+255
-                float v = __uint_as_float(vu[j]);
-                if (p.bias_base) v = p.mimic ? round_dt<DT>(round_dt<DT>(v) + bias1) : v + bias1;
-                if (p.ksplit > 1) atomicAdd(dst + BLOCK_M, v); else dst[BLOCK_M] = v;
-              }
+      for (int h = 0; h < 2; ++h) {
+        const int r = ra + 8 * h;
+        mrow[h] = t.m0 + r;
+        row_ok[h] = mrow[h] < p.M && r < m_rows;
+        row2_ok[h] = DUAL && mrow[h] + BLOCK_M < p.M;   // dual_m: second accumulator = rows m0+128..m0+255
+        if (p.bias_base) {
+          const uint16_t* bp = reinterpret_cast<const uint16_t*>(p.bias_base) + (size_t)t.slot * p.bias_slot_elems + p.bias_off;
+          if (row_ok[h]) bias0[h] = Half16<DT>::to_f(bp[mrow[h]]);
+          if (row2_ok[h]) bias1[h] = Half16<DT>::to_f(bp[mrow[h] + BLOCK_M]);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int h = i >> 1;
+          const int c = cb + 8 * j + (i & 1);
+          if (c >= t.ncols) continue;
+          const int m = mrow[h];
+          if (p.epi == EPI_LINEAR_F32) {
+            float* dst = reinterpret_cast<float*>(p.out) + (size_t)(t.row0 + c) * p.ld_out + m;
+            if (row_ok[h]) {
+              float v = acc0[4 * j + i];
+              if (p.bias_base) v = p.mimic ? round_dt<DT>(round_dt<DT>(v) + bias0[h]) : v + bias0[h];   // matmul, then `+ bias`
+              if (p.ksplit > 1) atomicAdd(dst, v); else *dst = v;
             }
-          }
-        } else {
-          uint16_t* out = reinterpret_cast<uint16_t*>(p.out);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (row_ok && c0 + j < t.ncols) {
-              float g = __uint_as_float(vg[j]);
-              float h;
-              if (DUAL) {
-                float u = __uint_as_float(vu[j]);
-                constexpr bool kFastAct = NT >= 256;
-                if (p.mimic) {   // reference rounding chain: each ATen op rounds to the model dtype; precise SiLU at every tile
-                  g = round_dt<DT>(g);   // width, so "reference numerics" does not depend on T (the MUFU form is NUMERICS_FP32 only)
-                  u = round_dt<DT>(u);
-                  h = round_dt<DT>(act_apply(g, p.act)) * u;
-                } else {
-                  h = ((kFastAct && p.act == ACT_SILU) ? silu_mufu(g) : act_apply(g, p.act)) * u;
-                }
+            if (DUAL && row2_ok[h]) {
+              float v = acc1[DUAL ? 4 * j + i : 0];
+              if (p.bias_base) v = p.mimic ? round_dt<DT>(round_dt<DT>(v) + bias1[h]) : v + bias1[h];
+              if (p.ksplit > 1) atomicAdd(dst + BLOCK_M, v); else dst[BLOCK_M] = v;
+            }
+          } else if (row_ok[h]) {
+            float g = acc0[4 * j + i];
+            float hv;
+            if (DUAL) {
+              float u = acc1[DUAL ? 4 * j + i : 0];
+              if (p.mimic) {   // reference rounding chain: each ATen op rounds to the model dtype
+                g = round_dt<DT>(g);
+                u = round_dt<DT>(u);
+                hv = round_dt<DT>(act_apply(g, p.act)) * u;
               } else {
-                if (p.mimic) g = round_dt<DT>(g);
-                if (p.bias_base) { g += bias0; if (p.mimic) g = round_dt<DT>(g); }
-                h = act_apply(g, p.act);
+                hv = act_apply(g, p.act) * u;
               }
-              out[(size_t)(t.row0 + c0 + j) * p.ld_out + m] = Half16<DT>::from_f(h);
+            } else {
+              if (p.mimic) g = round_dt<DT>(g);
+              if (p.bias_base) { g += bias0[h]; if (p.mimic) g = round_dt<DT>(g); }
+              hv = act_apply(g, p.act);
             }
+            reinterpret_cast<uint16_t*>(p.out)[(size_t)(t.row0 + c) * p.ld_out + m] = Half16<DT>::from_f(hv);
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == Cfg::ACC_STAGES) { acc = 0; acc_phase ^= 1; }
     }
   }
 
-  // ---- end of the phase: every role of this CTA is done with the ring, the barriers and the accumulators
-  tc_fence_before();
+  // ---- end of the phase: every role of this CTA is done with the ring and the barriers
   __syncthreads();
 }
 
-// after the last phase of a kernel: timeline, the expert-parallel "done" signal, TMEM release
+// after the last phase of a kernel: timeline and the expert-parallel "done" signal
 template <int MC>
-__device__ __forceinline__ void gemm_finish(const GemmParams& p, uint32_t tmem_base, int tmem_cols) {
-  const int warp = threadIdx.x >> 5;
+__device__ __forceinline__ void gemm_finish(const GemmParams& p) {
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
   if (p.ep_signal && threadIdx.x == 0) {
     // the CTA's output stores / reductions (all threads, ordered before this point by the barrier that ended the phase) become
@@ -435,55 +412,36 @@ __device__ __forceinline__ void gemm_finish(const GemmParams& p, uint32_t tmem_b
       for (int r = 0; r < p.ep_nranks; ++r) st_relaxed_sys(p.ep_peer_done_flag[r] + p.ep_rank, e);   // themselves go out back to back
     }
   }
-  if (MC > 1) cluster_sync_all();   // no CTA leaves while a peer may still multicast / commit into its shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
+  if (MC > 1) cluster_sync_all();   // no CTA leaves while a peer may still multicast into or arrive on its shared memory
 }
 
 __device__ __forceinline__ uint8_t* smem_aligned(uint8_t* raw) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
-}
-// allocate `cols` TMEM columns (warp 2) and hand the base address to every thread
-__device__ __forceinline__ uint32_t tmem_setup(uint32_t* slot, int cols) {
-  if ((threadIdx.x >> 5) == 2) {
-    tmem_alloc(slot, cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  return *slot;
 }
 
 template <int NT, bool DUAL, int DT, int MC>
 __global__ void __launch_bounds__((GemmCfg<NT, DUAL>::THREADS), 1)
 grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                        const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using Cfg = GemmCfg<NT, DUAL>;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t s_tmem;
   uint8_t* smem = smem_aligned(smem_raw);
   if (p.tl && threadIdx.x == 0) tl_min(p.tl);
   // pdl_edge: this grid may be resident long before its predecessor finishes (expert parallel: the gate/up GEMM arrives behind the
   // routing kernel to prefetch weights into L2).  Its successor reads state the predecessor publishes (dispatch epoch, row
   // counters) in ITS prologue, so it must not be released before this grid has passed its own wait: gemm_body triggers then.
   if (!p.pdl_edge) pdl_launch();
-  const uint32_t tmem_base = tmem_setup(&s_tmem, Cfg::TMEM_COLS);
   GridBar nobar{nullptr, 0};
-  gemm_body<NT, DUAL, DT, MC>(tmA0, tmA1, tmB, p, smem, tmem_base, DEP_PDL, nobar, (int)gridDim.x);
-  gemm_finish<MC>(p, tmem_base, Cfg::TMEM_COLS);
+  gemm_body<NT, DUAL, DT, MC>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
+  gemm_finish<MC>(p);
 }
 
 #ifdef B2M_ENABLE_FUSED_FFN
-// (Experiment, measured and NOT part of the default library: Mixtral decode 12.89 vs 12.84 ms/step, DeepSeek-V2-Lite decode
-// 5.04 vs 4.75 ms/step -- a persistent barrier kernel keeps the side-stream shared-expert GEMMs off the SMs --, expert
-// parallel N=2 8.51 vs 8.47 ms/step; profiles/r02c_*.json.  Build with -DB2M_ENABLE_FUSED_FFN and run with B2M_FUSED_FFN=1.)
+// (Experiment, NOT part of the default library: a persistent barrier kernel keeps the side-stream shared-expert GEMMs off the
+// SMs.  Build with -DB2M_ENABLE_FUSED_FFN and run with B2M_FUSED_FFN=1.)
 // Fused expert FFN for the HBM-bound (decode) regime: gate/up GEMM + SwiGLU, grid-wide barrier, down GEMM in ONE persistent
 // kernel.  What it removes from every layer: a kernel boundary on the critical path -- the down GEMM's CTAs could only become
-// resident when the gate/up CTAs had left their SMs (both want all shared memory), so its TMEM/barrier set-up, tile tables and
-// first pipeline fill were exposed (measured ~15 us per layer at every N, profiles/r02_ep*_timeline_regions.log).  Here the
+// resident when the gate/up CTAs had left their SMs (both want all shared memory), so its barrier set-up, tile tables and
+// first pipeline fill were exposed.  Here the
 // CTA keeps its resources, re-arms its barriers, starts streaming the down projection's weights at once and only its token
 // tiles wait for the grid barrier.  Needs every CTA resident (persistent grid <= #SMs, one CTA per SM: true by construction)
 // and no second barrier-kernel running beside it.
@@ -495,17 +453,16 @@ fused_ffn_kernel(const __grid_constant__ CUtensorMap tmGate, const __grid_consta
                  int up_ctas) {
   using CfgU = GemmCfg<NT, true>;
   using CfgD = GemmCfg<NT, false>;
-  constexpr int TMEM_COLS = CfgU::TMEM_COLS > CfgD::TMEM_COLS ? CfgU::TMEM_COLS : CfgD::TMEM_COLS;
+  static_assert(CfgU::THREADS == CfgD::THREADS, "both phases run on the same block");
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t s_tmem;
   __shared__ int s_gen;
   uint8_t* smem = smem_aligned(smem_raw);
   if (up.tl && threadIdx.x == 0) tl_min(up.tl);
   pdl_launch();
   if (threadIdx.x == 0) s_gen = *reinterpret_cast<volatile int*>(gbar_word + 1);   // moves only after every CTA of this grid arrived
-  const uint32_t tmem_base = tmem_setup(&s_tmem, TMEM_COLS);
+  __syncthreads();
   GridBar gb{gbar_word, s_gen};
-  gemm_body<NT, true, DT, 1>(tmGate, tmUp, tmBup, up, smem, tmem_base, DEP_PDL, gb, up_ctas);
+  gemm_body<NT, true, DT, 1, false>(tmGate, tmUp, tmBup, up, smem, DEP_PDL, gb, up_ctas);
   if (threadIdx.x == 0) {
     if (up.tl) tl_max(up.tl + 2);
     if (dn.tl) tl_min(dn.tl);
@@ -516,8 +473,8 @@ fused_ffn_kernel(const __grid_constant__ CUtensorMap tmGate, const __grid_consta
       asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(gbar_word + 1), "r"(gb.gen + 1) : "memory");
     }
   }
-  gemm_body<NT, false, DT, 1>(tmDown, tmDown, tmBdn, dn, smem, tmem_base, DEP_GRID, gb, (int)gridDim.x);
-  gemm_finish<1>(dn, tmem_base, TMEM_COLS);
+  gemm_body<NT, false, DT, 1, false>(tmDown, tmDown, tmBdn, dn, smem, DEP_GRID, gb, (int)gridDim.x);
+  gemm_finish<1>(dn);
 }
 
 #endif  // B2M_ENABLE_FUSED_FFN
@@ -592,6 +549,12 @@ static cudaError_t launch_tc(const CUtensorMap& a0, const CUtensorMap& a1, const
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return e;
+    // the consumers' setmaxnreg.inc is granted from the registers the block was launched with: a kernel compiled to fewer
+    // registers per thread than the split assumes would wait forever -> refuse to launch it
+    cudaFuncAttributes fa;
+    e = cudaFuncGetAttributes(&fa, kern);
+    if (e != cudaSuccess) return e;
+    if (fa.numRegs != Cfg::LAUNCH_REGS) return cudaErrorInvalidConfiguration;
     attr_done = true;
   }
   if (MC > 1) grid -= grid % MC;
@@ -651,7 +614,8 @@ static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const C
     B2M_CASE(32)
     B2M_CASE(64)
     B2M_CASE(128)
-    B2M_CASE(256)
+    case 256:   // single projections only (GemmCfg)
+      return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT>(a0, a1, b, p, grid, st);
     default:
       return cudaErrorInvalidValue;
   }
@@ -660,7 +624,7 @@ static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const C
 
 #ifdef B2M_ENABLE_MC2
 // 2-CTA multicast variant (prefill: NT = 128, several token tiles per expert); a0/a1 must be the 64-row-box maps.
-// Measured: no gain on B200 -> not instantiated in the default build (-DB2M_ENABLE_MC2 brings it back).
+// Not instantiated in the default build (-DB2M_ENABLE_MC2 brings it back).
 cudaError_t launch_grouped_gemm_tc_mc2(int dtype, bool dual, const CUtensorMap& a0h, const CUtensorMap& a1h,
                                        const CUtensorMap& b, const GemmParams& p, int grid, cudaStream_t st) {
   if (p.E > MAX_E) return cudaErrorInvalidValue;
@@ -682,7 +646,7 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
 
 cudaError_t launch_grouped_gemm_simt(int dtype, const void* arena, size_t slot_elems, size_t offA0, size_t offA1,
                                      const void* B, int ldb, const GemmParams& p, bool dual, cudaStream_t st) {
-  const int grid = 148 * 8;
+  const int grid = H100_SMS * 8;   // grid-stride loop
   if (dtype == DT_BF16)
     grouped_gemm_simt_kernel<DT_BF16><<<grid, 256, 0, st>>>((const uint16_t*)arena, slot_elems, offA0, offA1,
                                                              (const uint16_t*)B, ldb, p, dual ? 1 : 0);
@@ -700,7 +664,7 @@ int gemm_tc_smem_bytes(int nt, bool dual) {
     case 32: return dual ? GemmCfg<32, true>::SMEM_BYTES : GemmCfg<32, false>::SMEM_BYTES;
     case 64: return dual ? GemmCfg<64, true>::SMEM_BYTES : GemmCfg<64, false>::SMEM_BYTES;
     case 128: return dual ? GemmCfg<128, true>::SMEM_BYTES : GemmCfg<128, false>::SMEM_BYTES;
-    case 256: return dual ? GemmCfg<256, true>::SMEM_BYTES : GemmCfg<256, false>::SMEM_BYTES;
+    case 256: return dual ? -1 : GemmCfg<256, false>::SMEM_BYTES;
   }
   return -1;
 }

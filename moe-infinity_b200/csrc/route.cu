@@ -150,9 +150,9 @@ __device__ __forceinline__ void gate_dot8_warp(const RouteParams& p, int t, int 
 // indices derived from it must match the reference's fp32 linear, so no reduced-precision tensor-core inputs).
 // A CTA owns 32 tokens (8 warps x GATE_TW) and walks (8-expert group, 256-element slice of H) chunks of the gate matrix:
 // each chunk (8 KB fp32 / 4 KB 16-bit) is staged ONCE per CTA in shared memory by cp.async (3-deep ring, one
-// __syncthreads per chunk) and used by all 8 warps for GATE_TW x 8 x 8 FMAs per lane.  The first version read the gate
-// rows per token straight from L2 (2 GB of L2 traffic per DeepSeek-V2-Lite layer at T=4096; 158 us); a register-only
-// variant with 4-8 tokens per warp was still L2-bound at ~6 TB/s (94-102 us).  Expert groups are split over blockIdx.y
+// __syncthreads per chunk) and used by all 8 warps for GATE_TW x 8 x 8 FMAs per lane.  Reading the gate rows per token
+// straight from L2 instead moves 2 GB of L2 traffic per DeepSeek-V2-Lite layer at T=4096, and a register-only variant
+// with 4-8 tokens per warp stays L2-bound.  Expert groups are split over blockIdx.y
 // when the token blocks alone would not fill the GPU.
 constexpr int GATE_TW = 4;
 constexpr int GATE_TOK_PER_CTA = 8 * GATE_TW;
@@ -1021,7 +1021,7 @@ cudaError_t launch_route(const RouteParams& p, cudaStream_t st) {
       const int nblocks = (p.T + GATE_TOK_PER_CTA - 1) / GATE_TOK_PER_CTA;
       // expert groups are split over blockIdx.y so that (rounds of resident CTAs) x (chunks per CTA) is smallest;
       // 2 CTAs fit per SM.  Ties -> fewer splits (each split re-reads the token rows).
-      const long long slots = 2LL * 148;
+      const long long slots = 2LL * H100_SMS;
       int gsplit = 1;
       long long best = -1;
       for (int g = 1; g <= ngroups; ++g) {
@@ -1251,7 +1251,7 @@ __global__ void cast_rows_kernel(const float* __restrict__ y, uint16_t* __restri
 cudaError_t launch_cast_rows(const float* y, void* out, size_t n, int dtype, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
   if (n % 8) return cudaErrorInvalidValue;
-  const int blocks = (int)((n / 8 + 255) / 256 < 148 * 8 ? (n / 8 + 255) / 256 : 148 * 8);
+  const int blocks = (int)((n / 8 + 255) / 256 < H100_SMS * 8 ? (n / 8 + 255) / 256 : H100_SMS * 8);
   if (dtype == DT_F32) return cudaMemcpyAsync(out, y, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
   if (dtype == DT_BF16) cast_rows_kernel<DT_BF16><<<blocks, 256, 0, st>>>(y, (uint16_t*)out, n);
   else if (dtype == DT_F16) cast_rows_kernel<DT_F16><<<blocks, 256, 0, st>>>(y, (uint16_t*)out, n);

@@ -7,7 +7,7 @@
 // (:123-212): a *synchronous* call that cuts the aligned byte range into 1 MiB preads, runs them on ONE worker thread
 // ("only one SSD device") and lets a high-priority request overtake low-priority ones between blocks.
 //
-// Same contract, different machine: an NVMe array feeding a B200 needs many requests in flight, so
+// Same contract, different machine: an NVMe array feeding a GPU needs many requests in flight, so
 //   * requests are asynchronous (ticket = submit, wait/poll later): the caller overlaps the read of chunk i+1 with the
 //     host->device copy of chunk i (api.cu: issue_copy of a store-backed expert);
 //   * a pool of worker threads (default 8) takes blocks (default 4 MiB) from two queues, high before low, so an on-demand

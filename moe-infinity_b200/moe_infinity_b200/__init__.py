@@ -1,4 +1,4 @@
-"""moe_infinity_b200 -- B200-native (sm_100a) MoE expert dispatch/offload hot path.
+"""moe_infinity_b200 -- H100-native (sm_90a) MoE expert dispatch/offload hot path.
 
 Drop-in for the one hot path of EfficientMoE/MoE-Infinity (router top-k -> permute -> grouped expert GEMM ->
 combine, plus HBM expert cache and prefetch).  Everything numerical runs in libb2m.so (hand-written CUDA);

@@ -127,7 +127,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            f"{LIB_PATH} is not built. Run `python -m moe_infinity_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is not built. Run `python -m moe_infinity_b200.build` (nvcc, sm_90a). "
             "This package has no CPU or PyTorch fallback for the MoE dispatch path.")
     lib = C.CDLL(LIB_PATH)
     for name, res, args in SYMBOLS:

@@ -1,4 +1,4 @@
-"""Build libb2m.so (sm_100a only) in-tree with nvcc.  `python -m moe_infinity_b200.build`."""
+"""Build libb2m.so (sm_90a only) in-tree with nvcc.  `python -m moe_infinity_b200.build`."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(PKG_DIR, "libb2m.so")
 SOURCES = ["grouped_gemm.cu", "route.cu", "ep.cu", "f32_path.cu", "tracer.cu", "store_reader.cpp", "api.cu"]
 HEADERS = ["b2m_common.cuh", "b2m_internal.h", "tile_walker.cuh", "ep_device.cuh",
            os.path.join("..", "..", "include", "b2m.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 OBJ_DIR = os.path.join(CSRC, "_obj")     # git-ignored (*.o); one object per translation unit, compiled in parallel
 

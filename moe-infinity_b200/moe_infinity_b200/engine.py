@@ -49,7 +49,7 @@ class MoEEngine:
                  cache_policy: int = L.CACHE_REFERENCE, lookahead_prefetch: bool = False, freq_alpha: float = 0.0):
         self.lib = L.load()
         if not torch.cuda.is_available():
-            raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if dtype not in _TORCH2INT:
             raise ValueError(f"unsupported dtype {dtype}")
         self.dtype = dtype

@@ -1,7 +1,7 @@
 """Activation-aware expert tracing / prediction / prefetch request building (host policy, P1-P4).
 
 Mirrors the reference's moe_infinity/memory/{expert_tracer,expert_predictor,expert_prefetcher}.py
-(same class and method names, same results) with two changes that matter on a B200:
+(same class and method names, same results) with two changes that matter on the GPU:
   * no device round trips: the reference keeps the trace library on cuda:0 and pays two host syncs per
     sequence per layer (expert_tracer.py:104,120,124); here the library is a NumPy array on the host and
     `find_most_similar` is one vectorised expression (the library is <= 1000 x L x E floats);

@@ -22,7 +22,7 @@ pin is made from outputs of the reference itself run in the dev container:
       with this module and tests/golden/*.pt hold their outputs (tests/golden/make_golden.py).  The Switch block runs on a
       4.x-order router shim (HF 5.5's router returns another tuple), which restates the transformers 4.x forward;
   (c) cache policy: oracle/policy_oracle.py is pinned on a trace recorded from the reference's real engine
-      (tests/golden/policy_ref_trace.json, tools/ref_engine_harness.py --mode policy on a B200).
+      (tests/golden/policy_ref_trace.json, tools/ref_engine_harness.py --mode policy).
 
 Determinism choices (the reference itself is nondeterministic, SURVEY §9 Q1):
   * experts are combined in ascending expert id (reference: thread completion order,

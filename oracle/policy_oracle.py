@@ -26,7 +26,7 @@ evicts a protected expert (it is dropped instead); an on-demand miss may, as a l
 
 Parity status: pinned for the on-demand path -- tests/golden/policy_ref_trace.json holds hit / resident-set sequences
 recorded from the reference's own compiled engine (oracle/_ref/prefetch_op.so driven by tools/ref_engine_harness.py
---mode policy on a B200); tests/test_oracle_policy_ref.py demands this oracle reproduce them and
+--mode policy); tests/test_oracle_policy_ref.py demands this oracle reproduce them and
 tests/test_gpu_offload.py demands the CUDA engine reproduce the oracle.  The prefetch side (protected candidates,
 evict-to-fit) has no reference test and pins our stated policy only.
 """

@@ -5,7 +5,7 @@ The Python half of the reference is built the same way as its C++ half (oracle/r
 sources where they lie under $REF, outputs only into oracle/_ref/ (git-ignored, travels to the GPU box with the
 snapshot).  For Python "compiled" means byte-compiled: every hot-path module becomes a sourceless `<module>.pyc` under
 oracle/_ref/pyref/, which `tests/shims/ref_loader.py` imports where /root/reference does not exist, so that the
-reference's own unmodified blocks can be executed on a B200 on top of this repository's `compat` objects
+reference's own unmodified blocks can be executed on the GPU on top of this repository's `compat` objects
 (tests/test_gpu_literal_blocks.py).  No reference source text is copied anywhere; the product package never reads
 oracle/_ref/.
 

@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "moe-infinity_b200"), os.path.join(ROOT, "tes
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")

@@ -35,7 +35,7 @@ def build() -> str | None:
     cuda_inc = os.path.join(os.path.dirname(os.path.dirname(nvcc)), "include")
     inc = ["-I", CSRC, "-I", os.path.join(ROOT, "include"), "-I", cuda_inc]
     api_o, k_o, r_o = (os.path.join(OUT, n) for n in ("api.o", "fake_kernels.o", "fake_cudart.o"))
-    subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-std=c++17", "-Xcompiler", "-fPIC",
+    subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-std=c++17", "-Xcompiler", "-fPIC",
                     "-cudart", "none", "-diag-suppress", "177", *inc, "-c", os.path.join(CSRC, "api.cu"), "-o", api_o],
                    check=True, capture_output=True)
     s_o = os.path.join(OUT, "store_reader.o")           # the product's disk-tier reader is host code: compiled as it is

@@ -44,8 +44,8 @@ cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 cudaError_t cudaGetDeviceProperties_v2(cudaDeviceProp* p, int) {
   std::memset(p, 0, sizeof *p);
-  std::strcpy(p->name, "simulated B200 (host)");
-  p->major = 10; p->minor = 0; p->multiProcessorCount = 148; p->totalGlobalMem = (size_t)g_total_mem;
+  std::strcpy(p->name, "simulated H100 (host)");
+  p->major = 9; p->minor = 0; p->multiProcessorCount = 132; p->totalGlobalMem = (size_t)g_total_mem;
   p->sharedMemPerBlockOptin = 227 * 1024;
   return cudaSuccess;
 }

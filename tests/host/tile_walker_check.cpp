@@ -91,7 +91,7 @@ int main(int argc, char** argv) {
     c.kblocks = U(1, 40);
     c.m_step = U(0, 1) ? 256 : 128;                      // dual_m pairs two 128-row tiles
     c.m_tiles = U(1, 6);
-    c.grid = U(0, 4) == 0 ? 148 : U(1, 40);
+    c.grid = U(0, 4) == 0 ? 132 : U(1, 40);
     if (c.MC == 2) c.grid = 2 * U(1, 20);
     // split-K factor as pick_ksplit (api.cu) produces it: every split non-empty
     c.ksplit = U(1, 8);

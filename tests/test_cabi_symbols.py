@@ -35,16 +35,16 @@ def test_config_struct_layout_matches_header(lib_built):
     assert _lib.Config.device_memory_ratio.offset % 8 == 0
 
 
-def test_library_has_blackwell_sass(lib_built):
+def test_library_has_hopper_sass(lib_built):
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", lib_built], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass, "tcgen05.mma missing"
+    assert "HGMMA" in sass, "wgmma missing"
     assert "UTMALDG" in sass, "TMA loads missing"
-    assert "LDTM" in sass, "tcgen05.ld missing"
-    assert "sm_100a" in sass
+    assert "SYNCS" in sass, "mbarrier waits missing"
+    assert "sm_90a" in sass
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

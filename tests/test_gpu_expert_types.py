@@ -40,6 +40,8 @@ def _second_expert(ws, seed):
     return [(torch.randn(w.shape, generator=g) * (0.3 if w.dim() == 1 else 0.08)).to(w.dtype) for w in ws]
 
 
+# id "tcgen05" = gemm_impl 0, the tensor-core product path (wgmma on sm_90a); the name is kept so the test
+# ids stay the same across GPU architectures
 @pytest.mark.parametrize("impl", [0, 1], ids=["tcgen05", "simt"])
 @pytest.mark.parametrize("name", HALF_CASES)
 def test_expert_type_outputs_match_reference_module(lib_built, name, impl):

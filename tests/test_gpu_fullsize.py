@@ -84,7 +84,7 @@ def test_fullsize_zero_and_scaling_properties(layer):
     x = torch.randn(T, H, device="cuda").to(DT)
     lg = torch.randn(T, E, device="cuda").to(DT)
     a = eng.forward(0, x, router_logits=lg).clone()
-    # the down projection is linear: tcgen05 path == CUDA-core cross-check path on the same rows
+    # the down projection is linear: wgmma path == CUDA-core cross-check path on the same rows
     from moe_infinity_b200 import MoEEngine
     cnt = eng.ws("counts", T).cpu()
     assert int(cnt.sum()) == T * K
@@ -166,8 +166,8 @@ def test_deepseek_v2_lite_fullsize_prefill_tiles_match_oracle(ds_layer):
 
 def test_mixtral_fullsize_prefill_tiles_match_oracle(lib_built):
     """One full-size Mixtral expert pair at a prefill-sized batch (T=2048 over 2 experts -> 2048 rows each = eight
-    256-token tiles), both numerics modes: reference (precise SiLU, 128-token gate/up tiles) and fp32 (MUFU SiLU in the
-    256-token instantiation, grouped_gemm.cu silu_mufu) against the CPU oracle on sampled tokens."""
+    256-token tiles), both numerics modes (128-token gate/up tiles, 256-token down-projection tiles) against the CPU oracle on
+    sampled tokens."""
     from moe_infinity_b200 import MoEEngine, _lib as L
     E2, T = 2, 2048
     g = torch.Generator().manual_seed(9)

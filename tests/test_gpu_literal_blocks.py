@@ -1,5 +1,5 @@
 """GPU: the reference's OWN, unmodified MoE blocks (moe_infinity/models/{mixtral,deepseek,switch_transformers,nllb_moe}.py, loaded
-through tests/shims/ref_loader.py from /root/reference or its byte-compiled staging oracle/_ref/pyref) running on a B200 on
+through tests/shims/ref_loader.py from a reference checkout or its byte-compiled staging oracle/_ref/pyref; skipped where neither exists) running on the GPU on
 top of this repository's plugin objects, constructed exactly the way moe_infinity/runtime/model_offload.py constructs the
 reference's (`prefetch_handle(prefix, ratio)`, `expert_dispatcher(E, L, dtype, expert_type, num_threads)` -- five positional
 arguments, :143-145, :471-477 -- then `offload` / `register_expert` / `set_expert_dispatcher`).  The block's Python (router

@@ -168,7 +168,7 @@ def test_unregistered_expert_is_an_error(lib_built):
 
 def test_cache_policy_matches_reference_engine_trace(lib_built):
     """The CUDA engine, driven through the reference-signature `expert_dispatcher` exactly like the reference engine was
-    when tests/golden/policy_ref_trace.json was recorded on a B200 (tools/ref_engine_harness.py --mode policy, protocol
+    when tests/golden/policy_ref_trace.json was recorded (tools/ref_engine_harness.py --mode policy, protocol
     "sequential"), reproduces the hit flags and resident sets of the reference's real GPUFetchFunc."""
     import json
     import os

@@ -153,6 +153,8 @@ def test_mixtral_routing_and_permute_golden(name, lib_built):
     check_permutation(eng, x.reshape(T, -1), T)
 
 
+# id "tcgen05" = gemm_impl 0, the tensor-core product path (wgmma on sm_90a); the name is kept so the test
+# ids stay the same across GPU architectures
 @pytest.mark.parametrize("gemm_impl", [0, 1], ids=["tcgen05", "simt"])
 @pytest.mark.parametrize("name", MIXTRAL)
 def test_mixtral_forward_golden(name, gemm_impl, lib_built):
@@ -187,6 +189,8 @@ def test_mixtral_fused_gate(name, lib_built):
     assert torch.all((o - r).abs() <= tol * r.abs() + tol * rms)
 
 
+# id "tcgen05" = gemm_impl 0, the tensor-core product path (wgmma on sm_90a); the name is kept so the test
+# ids stay the same across GPU architectures
 @pytest.mark.parametrize("gemm_impl", [0, 1], ids=["tcgen05", "simt"])
 @pytest.mark.parametrize("name", DEEPSEEK)
 def test_deepseek_forward_golden(name, gemm_impl, lib_built):

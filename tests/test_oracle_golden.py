@@ -1,7 +1,6 @@
-"""CPU: the oracle against the committed golden vectors, and against the literal reference block files executed from
-/root/reference (dev container) or from their byte-compiled staging oracle/_ref/pyref (anywhere the snapshot travels)."""
+"""CPU: the oracle against the committed golden vectors, which the literal reference block files produced
+(tests/golden/make_golden.py)."""
 import os
-import sys
 
 import pytest
 import torch
@@ -10,10 +9,6 @@ from oracle import moe_oracle as O
 import make_golden as G
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims"))
-import ref_loader  # noqa: E402
-
-needs_reference = pytest.mark.skipif(not ref_loader.available(), reason="neither /root/reference nor oracle/_ref/pyref present")
 
 
 def _load(name):
@@ -86,63 +81,55 @@ def test_empty_and_single_expert_edge_cases():
     assert r.topk_idx.tolist() == [[0, 1]] * 5 and O.tied_tokens(r.scores, 2).all()
 
 
-@needs_reference
 @pytest.mark.parametrize("name", ["mixtral_mini_bf16", "mixtral_ragged_bf16"])
 def test_literal_reference_block_equals_oracle(name):
-    ns = ref_loader.load()
+    """The reference's own SyncMixtralSparseMoeBlock produced the fixture (tests/golden/make_golden.py); the oracle must
+    reproduce its router logits and, on untied tokens, its output bit for bit."""
+    fx = _load(name)
+    assert fx["source"] == "literal"
     c = G.build_mixtral(name)
-    l_out, l_logits = G.run_literal_mixtral(ns, c["H"], c["I"], c["E"], c["k"], c["hidden"], c["gate"], c["experts"])
     o_out, o_logits, r = O.mixtral_block(c["hidden"], c["gate"], c["experts"], c["k"])
-    assert torch.equal(l_logits, o_logits)
+    assert torch.equal(fx["router_logits"], o_logits)
     ok = ~O.tied_tokens(r.scores, c["k"])
-    assert torch.equal(l_out.reshape(-1, c["H"])[ok], o_out.reshape(-1, c["H"])[ok])
+    assert torch.equal(fx["out"].reshape(-1, c["H"])[ok], o_out.reshape(-1, c["H"])[ok])
 
 
-@needs_reference
 def test_literal_deepseek_block_equals_oracle():
-    ns = ref_loader.load()
+    """The reference's own DeepseekMoEBlock (literal MoEGate) produced the fixture; the oracle reproduces it on untied tokens."""
     name = "deepseek_group_bf16"
+    fx = _load(name)
+    assert fx["source"] == "literal"
     c = G.build_deepseek(name)
-    l_out = G.run_literal_deepseek(ns, c["H"], c["I"], c["E"], c["k"], c["n_shared"], c["hidden"], c["gate"], c["experts"],
-                                   c["shared"], c["topk_method"], c["n_group"], c["topk_group"], c["norm_topk_prob"],
-                                   c["routed_scaling_factor"])
     kw = {k: c[k] for k in ("topk_method", "n_group", "topk_group", "norm_topk_prob", "routed_scaling_factor")}
     o_out, r = O.deepseek_block(c["hidden"], c["gate"], c["experts"], c["k"], c["shared"], **kw)
     ok = ~O.tied_tokens(r.scores, c["k"])
-    assert torch.equal(l_out.reshape(-1, c["H"])[ok], o_out.reshape(-1, c["H"])[ok])
+    assert torch.equal(fx["out"].reshape(-1, c["H"])[ok], o_out.reshape(-1, c["H"])[ok])
 
 
-@needs_reference
 @pytest.mark.parametrize("name", list(G.SWITCH_CASES))
 def test_literal_switch_block_equals_oracle(name):
     """A6 pin: the reference's own SyncSwitchTransformersSparseMLP (switch_transformers.py:41-113) on the 4.x-order router
-    shim, bit for bit against the oracle -- outputs, router logits, expert index, including capacity drops."""
-    ns = ref_loader.load()
-    c = G.build_switch(name)
-    l_out, l_logits, l_index = G.run_literal_switch(ns, c["H"], c["I"], c["E"], c["capacity"], c["hidden"], c["gate"],
-                                                    c["experts"])
-    o_out, (o_logits, o_index), mask = O.switch_block(c["hidden"], c["gate"], c["experts"], c["capacity"])
-    assert torch.equal(l_logits.float(), o_logits.float())
-    assert torch.equal(l_index, o_index)
-    assert torch.equal(l_out, o_out)
+    shim produced the fixture; the oracle matches it bit for bit -- outputs, router logits, expert index, including
+    capacity drops."""
     fx = _load(name)
-    assert fx["source"] == "literal" and torch.equal(fx["out"], l_out)
+    assert fx["source"] == "literal"
+    c = G.build_switch(name)
+    o_out, (o_logits, o_index), mask = O.switch_block(c["hidden"], c["gate"], c["experts"], c["capacity"])
+    assert torch.equal(fx["router_logits"].float(), o_logits.float())
+    assert torch.equal(fx["expert_index"], o_index)
+    assert torch.equal(fx["out"], o_out)
 
 
-@needs_reference
 @pytest.mark.parametrize("name", list(G.NLLB_CASES))
 def test_literal_nllb_block_reproduces_its_golden(name):
     """The reference's own SyncNllbMoeSparseMLP (nllb_moe.py:20-115; HF's top-2 router on its 4.x contract) with the oracle's
-    NllbMoeDenseActDense behind dispatch_local reproduces the committed fixture bit for bit -- here and from the byte-compiled
-    staging -- and its output is the literal combine of the oracle's per-expert results (the part a plugin must get right)."""
-    if not hasattr(ref_loader.load(), "nllb"):
-        pytest.skip("the NLLB block could not be imported")
-    ns = ref_loader.load()
-    c = G.build_nllb(name)
-    out, probs, top1 = G.run_literal_nllb(ns, c["H"], c["I"], c["E"], c["capacity"], c["hidden"], c["gate"], c["experts"])
+    NllbMoeDenseActDense behind dispatch_local produced the fixture; its output is the literal combine of the oracle's
+    per-expert results under the recorded router probabilities (the part a plugin must get right)."""
     fx = _load(name)
-    assert fx["kind"] == "nllb" and torch.equal(fx["out"], out) and torch.equal(fx["router_probs"], probs)
-    assert torch.equal(fx["top1"], top1)
+    assert fx["kind"] == "nllb" and fx["source"] == "literal"
+    c = G.build_nllb(name)
+    assert torch.equal(c["hidden"], fx["hidden"])
+    out, probs = fx["out"], fx["router_probs"]
     # restated combine: per expert, weights * output added in ascending expert order; untouched elements keep the input
     x = c["hidden"].reshape(-1, c["H"])
     w = probs.reshape(-1, c["E"])

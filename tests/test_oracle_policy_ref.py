@@ -1,6 +1,6 @@
 """CPU: the cache-policy oracle and the host logic of csrc/api.cu against a trace RECORDED FROM THE REFERENCE'S OWN ENGINE.
 
-tests/golden/policy_ref_trace.json was produced on a B200 by tools/ref_engine_harness.py --mode policy: the reference's
+tests/golden/policy_ref_trace.json was produced by tools/ref_engine_harness.py --mode policy: the reference's
 compiled `prefetch_op.so` (core/parallel/expert_dispatcher.cpp GPUFetchFunc :191-307, Node::SetDevice) replayed a seeded
 sequence of (layer, active experts) requests with an HBM budget of `slots` experts; for every dispatched expert the
 harness stored the `hit` flag wait_expert() returned (:219,301) and the set of GPU-resident experts afterwards

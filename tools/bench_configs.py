@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Secondary measurements for the BASELINE.json configs that are not the headline bench line
-(bench.py keeps the driver contract; this script writes profiles/<tag>_configs.json).
+(bench.py prints the headline line; this script writes the secondary configurations to --out).
 
   prefill  : Mixtral-8x7B, T = 8*2048 = 16384 tokens through ONE MoE layer (tensor-core bound), TFLOP/s
   offload  : Mixtral-8x7B shapes, reduced depth, half of the experts HBM-resident (config 3 in miniature:
@@ -112,7 +112,7 @@ def deepseek(T, iters=20):
 
 
 def torch_gpu_reference(layers=4, T=8, iters=20):
-    """R-torch-gpu (BASELINE.md §4.3): what plain HF-style PyTorch gives on the same B200 for the same path --
+    """R-torch-gpu (BASELINE.md §4.3): what plain HF-style PyTorch gives on the same GPU for the same path --
     softmax/topk + per-expert index/matmul loop + index_add, ATen/cuBLAS kernels, eager launches.  Written out here
     (not the oracle): this is a measurement of the library path the reference itself calls on the GPU
     (core/parallel/expert_module.cpp:171-175 via torch::matmul), without its offload engine."""
@@ -236,7 +236,7 @@ def offload(layers=8, steps=24, prefetch=True, resident_frac=127 / 256, skew=1.0
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="h2d,torchgpu,prefill,deepseek,offload")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "configs.json"))
+    ap.add_argument("--out", default="configs.json")
     a = ap.parse_args()
     res = {}
     what = a.what.split(",")

@@ -1,5 +1,6 @@
 import sys, os
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/moe-infinity_b200"); sys.path.insert(0, "/root/repo/tools")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "moe-infinity_b200")); sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch, bench_configs as B
 from moe_infinity_b200 import MoEEngine, _lib as L
 Hh, I, E, k, Lr, T = 2048, 1408, 64, 6, 4, int(os.environ.get("DS_T", "16"))

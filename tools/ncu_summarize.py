@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Summarise ncu artefacts brought back in gpurun_out/ into small text/JSON files under profiles/.
+"""Summarise Nsight Compute artefacts into small text/JSON files.
 
-  python tools/ncu_summarize.py launches gpurun_out/launches.csv profiles/r01_launches.txt
-  python tools/ncu_summarize.py full gpurun_out/prof_k3.ncu-rep profiles/r01_k3_k4_full.txt [traffic.json kernel-substr]
+  python tools/ncu_summarize.py launches launches.csv launches.txt
+  python tools/ncu_summarize.py full prof_k3.ncu-rep k3_k4_full.txt [traffic.json kernel-substr]
 """
 import collections
 import csv

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Offline study of BASELINE config 3 (Mixtral-8x7B, device_memory_ratio 0.25 -> 127 of 256 experts HBM resident):
+"""Offline study of BASELINE config 3 (Mixtral-8x7B, device_memory_ratio 0.25 -> 56 of 256 experts resident in 80 GB HBM):
 miss counts of cache policies on the SURVEY §8(d) decode trace (per-layer Zipf-skewed gates, sticky hidden states),
 computed on the CPU with oracle/policy_oracle.py -- the same policy code the CUDA engine is tested against.
 
-Time model: the step is bound by the host->device link (one Mixtral expert = 352 MB = 6.4 ms at 55 GB/s; the MoE math of
-a whole step is 13 ms), so ms/step ~= misses/step x 6.4 ms; a policy can only win by MOVING FEWER BYTES.
+Time model: the step is bound by the host->device link (one Mixtral expert = 352 MB, 6.4 ms at the default --link-gbs 55,
+an assumed PCIe Gen5 x16 rate, not a measurement; the MoE math of a step is far shorter), so ms/step ~= misses/step x the
+copy time of one expert; a policy can only win by MOVING FEWER BYTES.
   lfu       the reference's on-demand policy (expert_dispatcher.cpp:227-266): evict min incache_visit_count
   belady    clairvoyant optimum (evict the resident expert whose next use is farthest): the floor
   pred:K    lfu + protected set = experts predicted for the next K layers from the previous step's routing of the same
@@ -113,8 +114,10 @@ def run_next_use(trace, L, E, slots, alpha=0.25, floor=0.02):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=128)
-    ap.add_argument("--slots", type=int, default=127)
+    ap.add_argument("--slots", type=int, default=56)
+    ap.add_argument("--link-gbs", type=float, default=55.0, help="assumed host->device bandwidth")
     a = ap.parse_args()
+    ms_per_miss = 3 * 4096 * 14336 * 2 / (a.link_gbs * 1e9) * 1e3
     L, E = 32, 8
     for skew, rho in ((0.0, 0.0), (1.0, 0.9), (2.0, 0.9), (1.0, 0.99)):
         tr = make_trace(L, E, steps=a.steps, skew=skew, rho=rho)
@@ -130,7 +133,7 @@ def main():
             row[f"next:{al}"] = run_next_use(tr, L, E, a.slots, alpha=al)["misses"]
         per_step = {k_: round(v / a.steps, 1) for k_, v in row.items()}
         print(f"skew={skew} rho={rho}: dispatches/step={disp / a.steps:.1f}  misses/step {per_step}  "
-              f"-> link-bound ms/step {{k: v*6.4}} = {{ {', '.join(f'{k_}: {v * 6.4:.0f}' for k_, v in per_step.items())} }}")
+              f"-> link-bound ms/step = {{ {', '.join(f'{k_}: {v * ms_per_miss:.0f}' for k_, v in per_step.items())} }}")
 
 
 if __name__ == "__main__":

@@ -26,7 +26,7 @@ Gotchas taken from the reference code (SURVEY §8 c.2):
   * any DLOG_FATAL aborts the process; never destroy the engine objects (destructors join threads blocked on condition
     variables) -> os._exit at the end.
 
-  python tools/ref_engine_harness.py --mode policy --out gpurun_out/policy_ref_trace.json
+  python tools/ref_engine_harness.py --mode policy --out policy_ref_trace.json
   python tools/ref_engine_harness.py --mode timing --layers 4 --tokens 8 --steps 16 --ratio 0.9
 """
 from __future__ import annotations
@@ -47,7 +47,7 @@ sys.path.insert(0, os.path.join(ROOT, "moe-infinity_b200"))
 def load_reference_engine():
     so = os.path.join(ROOT, "oracle", "_ref", "prefetch_op.so")
     if not os.path.exists(so):
-        raise SystemExit(f"{so} missing: make -C oracle/ref_build -f Makefile.engine (needs /root/reference)")
+        raise SystemExit(f"{so} missing: make -C oracle/ref_build -f Makefile.engine (needs the reference tree)")
     import torch  # noqa: F401  (libtorch first)
     spec = importlib.util.spec_from_file_location("prefetch_op", so)
     mod = importlib.util.module_from_spec(spec)
@@ -76,8 +76,7 @@ def _accepts_o_direct(d: str) -> bool:
 def pick_store_dir(want: str, need_bytes: int) -> str:
     """First candidate directory that accepts O_DIRECT and has room; else re-exec under the no-O_DIRECT preload shim."""
     import shutil
-    cands = [want, "/var/tmp/b2m_ref_store", "/root/b2m_ref_store", "/tmp/b2m_ref_store",
-             os.path.join(ROOT, "gpurun_out", "ref_store"), "/dev/shm/b2m_ref_store"]
+    cands = [want, "/var/tmp/b2m_ref_store", "/tmp/b2m_ref_store", "/dev/shm/b2m_ref_store"]
     preload = "libnodirect.so" in os.environ.get("LD_PRELOAD", "")
     for d in cands:
         if not d:
@@ -260,8 +259,8 @@ def mode_policy(args):
             res = ref.d.wait_expert()
             hits = {int(e): int(h) for _, _, e, h in res}
             out["batch"].append({"rep": rep, "n": n, "layer": l, "hits": [hits[e] for e in act], "resident_after": ref.resident()})
-    path = args.out or os.path.join(ROOT, "gpurun_out", "policy_ref_trace.json")
-    os.makedirs(os.path.dirname(path), exist_ok=True)
+    path = args.out or "policy_ref_trace.json"
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     with open(path, "w") as f:
         json.dump(out, f)
     print(json.dumps({"mode": "policy", "out": path, "dispatches": len(out["sequential"]),
@@ -311,8 +310,8 @@ def mode_timing(args):
         else:
             # one expert per enqueue/wait.  Needed whenever the engine evicts: GPUFetchFunc's victim scan try_locks EVERY
             # node (expert_dispatcher.cpp:239-245) while the Python thread is still enqueueing the layer's other experts,
-            # whose own try_lock then fails -> DLOG_FATAL -> abort (:127-132).  Observed on a B200 with 352 MB experts
-            # (profiles/r02_ref_engine_offload_batch_abort.log); the single fetch thread serialises the copies anyway.
+            # whose own try_lock then fails -> DLOG_FATAL -> abort (:127-132).  Observed with 352 MB experts
+            # the single fetch thread serialises the copies anyway.
             results = []
             for e in active:
                 d.set_inputs(x, mask)

@@ -6,7 +6,8 @@
 
 Decode is HBM bound: per layer the weights of the A *distinct activated* experts are streamed once,
 E[A] = E * (1 - (1 - k/E)^T) for uniform routing; prefill is tensor bound: 6*H*I FLOP per (token, expert).
-Peaks come from MEASURED_PEAKS.json (driver-written) when present, else the fallbacks of the B200 profiling guide."""
+Peaks are NVIDIA's data-sheet figures of the H100 card named by --card (default sxm; a card run below its rated power
+reaches less)."""
 from __future__ import annotations
 
 import argparse
@@ -21,15 +22,11 @@ MODELS = {
 }
 
 
-def peaks():
-    p = dict(hbm_gbs=7700.0 * 0.85, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            m = json.load(f)
-        p.update(hbm_gbs=m["hbm_gbs"], bf16_tflops_sustained=m.get("bf16_tflops_sustained", m.get("bf16_tflops")),
-                 source="MEASURED_PEAKS.json")
-    return p
+PEAKS = {
+    "sxm": dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="H100 SXM data sheet (HBM3, dense bf16)"),
+    "pcie": dict(hbm_gbs=2000.0, bf16_tflops=756.0, source="H100 PCIe data sheet (HBM2e, dense bf16)"),
+    "nvl": dict(hbm_gbs=3900.0, bf16_tflops=835.0, source="H100 NVL data sheet (HBM3, dense bf16)"),
+}
 
 
 def layer(model: dict, T: int, gpus: int = 1):
@@ -47,12 +44,12 @@ def layer(model: dict, T: int, gpus: int = 1):
                 expert_bytes=expert_bytes)
 
 
-def report(name: str, T: int, gpus: int):
-    m, p = MODELS[name], peaks()
+def report(name: str, T: int, gpus: int, card: str = "sxm"):
+    m, p = MODELS[name], PEAKS[card]
     lay = layer(m, T, gpus)
     L = m["L"]
     t_hbm = lay["bytes"] / (p["hbm_gbs"] * 1e9)
-    t_tc = lay["flops"] / (p["bf16_tflops_sustained"] * 1e12)
+    t_tc = lay["flops"] / (p["bf16_tflops"] * 1e12)
     bound = "hbm" if t_hbm >= t_tc else "tensor"
     t = max(t_hbm, t_tc)
     out = dict(model=name, tokens_per_gpu=T, gpus=gpus, active_experts_per_rank=round(lay["active_experts"], 2),
@@ -67,16 +64,17 @@ def main():
     ap.add_argument("--model", choices=sorted(MODELS))
     ap.add_argument("--tokens", type=int, default=8)
     ap.add_argument("--gpus", type=int, default=1)
+    ap.add_argument("--card", choices=sorted(PEAKS), default="sxm")
     a = ap.parse_args()
     if a.model:
-        print(json.dumps(report(a.model, a.tokens, a.gpus), indent=1))
+        print(json.dumps(report(a.model, a.tokens, a.gpus, a.card), indent=1))
         return
     rows = [("mixtral", 8, 1), ("mixtral", 8, 2), ("mixtral", 8, 4), ("mixtral", 8, 8), ("mixtral", 16384, 1),
             ("deepseek_v2_lite", 16, 1), ("deepseek_v2_lite", 4096, 1), ("deepseek_v2_lite", 65536, 1)]
     print(f"{'model':18s} {'T/gpu':>6s} {'gpus':>4s} {'A/rank':>7s} {'GB/step':>9s} {'TFLOP/step':>11s} {'bound':>7s} "
           f"{'min ms/step':>12s} {'max tok/s':>11s}")
     for name, T, g in rows:
-        r = report(name, T, g)
+        r = report(name, T, g, a.card)
         print(f"{name:18s} {T:6d} {g:4d} {r['active_experts_per_rank']:7.2f} {r['bytes_per_step'] / 1e9:9.2f} "
               f"{r['flops_per_layer'] * MODELS[name]['L'] / 1e12:11.2f} {r['bound']:>7s} {r['min_ms_per_step']:12.3f} "
               f"{r['max_tokens_per_s']:11.0f}")
