@@ -100,7 +100,14 @@ typedef struct b2m_config {
                                  (core/memory/memory_pool.cpp:150-158): slots = ratio * total HBM / expert bytes */
   int32_t max_inflight_prefetch; /* concurrent prefetch copies on the side stream (default 2) */
   int32_t h2d_chunk_bytes;  /* H2D copy granularity in bytes (0 = whole expert in one cudaMemcpyAsync) */
-  int32_t gemm_impl;        /* 0 = wgmma tensor cores (product); 1 = CUDA-core cross-check kernel (bring-up only) */
+  int32_t gemm_impl;        /* 0 = wgmma tensor cores (product); 1 = CUDA-core cross-check kernel (bring-up only);
+                               2 = wgmma tensor cores reading the bf16 slots only.
+                               With 0, the decode GEMMs (<= 64-token tiles) of an all-resident, single-rank bf16 context read the
+                               routed experts from a lossless 12-bit packed copy beside the bf16 slots (0.76 of their bytes,
+                               csrc/weight_pack.cuh; results are bit-identical), allocated by the first eager forward that packs if 2 GiB of
+                               device memory stay free.  A slot is packed by the second eager forward of its layer after
+                               b2m_make_resident(flags & 2), b2m_expert_dev_ptr or a host->device staging (the first one runs as
+                               without the copy); forwards captured into a graph before that read it as bf16.  2 never allocates the copy (frees that HBM). */
   int32_t cache_policy;     /* B2M_CACHE_* : on-demand budget accounting */
   int32_t lookahead_prefetch; /* 1 | 2 (offload mode, T <= 256): every routing call also applies the NEXT layer's router weight
                                (b2m_set_gate) to this layer's input and reads the predicted expert counts back with this

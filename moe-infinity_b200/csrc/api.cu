@@ -179,6 +179,19 @@ struct b2m_ctx {
 
   int cur_ksplit = 1, cur_nt = 16, cur_nt_dn = 16, cur_T = 0;   // token-tile widths of the up (K3) and down (K4) GEMMs
   bool ep_mode = false;       // experts of other ranks are simply absent (never an error)
+  // 12-bit packed copy of the routed arena (weight_pack.cuh; same slot index), read by the decode GEMMs.  Allocated by the first
+  // eager forward that packs, if the device keeps PK_RESERVE free beside it.  d_ok[slot]: bit b = matrix b (gate, up, down)
+  // of the slot has a current packed copy.  A slot is stale from the moment a caller may write it (its device flag is cleared
+  // in stream order then) until an eager forward of its layer packs it: the second one after the write, so the forward that
+  // directly follows a weight load runs exactly as it would without the packed copy (no allocation, no extra device work).
+  struct Packed {
+    int state = 0;              // 0 = not allocated yet, 1 = allocated, -1 = not available in this context
+    uint8_t* base = nullptr;
+    int* d_ok = nullptr;
+    size_t slot_bytes = 0;
+    size_t off[3] = {0, 0, 0};  // packed gate, up, down inside a packed slot
+    std::vector<uint8_t> dirty; // [nslots] PK_WRITTEN / PK_SEEN (one eager forward since the write) / 0 = packed or never
+  } pk;
   // device-side tracer / predictor (b2m_trace_*)
   struct Trace {
     int capacity = 0, max_seqs = 0, persistent = 0, auto_prefetch = 0;
@@ -366,6 +379,55 @@ cudaEvent_t next_ring_event(b2m_ctx* c, int* idx) {
   return e;
 }
 
+// ---------------- packed weights ----------------
+constexpr size_t PK_RESERVE = 2ull << 30;   // device memory left free beside the packed copy
+enum : uint8_t { PK_SEEN = 1, PK_WRITTEN = 2 };
+size_t pk_matrix_rows(const ExpertShape& s, int m) { return m == 2 ? s.H : (m == 1 && !s.dual) ? 0 : s.I; }
+size_t pk_matrix_cols(const ExpertShape& s, int m) { return m == 2 ? s.I : s.H; }
+// contexts whose routed experts the decode GEMMs may read from a packed copy: all resident, bf16 tensor cores (gemm_impl 0),
+// one rank
+bool pk_eligible(const b2m_ctx* c) {
+  return c->cfg.gemm_impl == 0 && !c->offload && c->cfg.dtype == B2M_DTYPE_BF16 && !c->ep_mode &&
+         c->pk.slot_bytes > 0;
+}
+// slot `slot` may be written by the caller from now on (on stream st): its packed copy is stale
+int pk_invalidate(b2m_ctx* c, int slot, cudaStream_t st) {
+  if (slot < 0 || c->pk.dirty.empty()) return B2M_OK;
+  c->pk.dirty[slot] = PK_WRITTEN;
+  if (c->pk.d_ok) CK(c, cudaMemsetAsync(c->pk.d_ok + slot, 0, sizeof(int), st));
+  return B2M_OK;
+}
+// the stale resident slots of `layer` that this eager call's gate/up GEMM launch packs (those seen by an earlier eager forward
+// since they were written); none while the stream is captured (their flags stay 0, the graph reads them as bf16)
+int pk_collect(b2m_ctx* c, int layer, cudaStream_t st, std::vector<int>* out) {
+  out->clear();
+  if (!pk_eligible(c) || c->pk.state < 0) return B2M_OK;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) cudaGetLastError();
+  if (cs != cudaStreamCaptureStatusNone) return B2M_OK;
+  const int E = c->cfg.num_experts;
+  for (int e = 0; e < E; ++e) {
+    const int slot = c->experts[(size_t)layer * E + e].slot;
+    if (slot < 0 || !c->pk.dirty[slot]) continue;
+    if (c->pk.dirty[slot] == PK_WRITTEN) c->pk.dirty[slot] = PK_SEEN;
+    else out->push_back(slot);
+  }
+  if (out->empty()) return B2M_OK;
+  if (c->pk.state == 0) {
+    c->pk.state = -1;
+    const size_t bytes = (size_t)c->arena.nslots * c->pk.slot_bytes;
+    size_t fr = 0, tot = 0;
+    CK(c, cudaMemGetInfo(&fr, &tot));
+    if (fr < bytes + PK_RESERVE + sizeof(int) * c->arena.nslots) { out->clear(); return B2M_OK; }
+    if (cudaMalloc((void**)&c->pk.base, bytes) != cudaSuccess) { cudaGetLastError(); out->clear(); return B2M_OK; }
+    CK(c, cudaMalloc((void**)&c->pk.d_ok, sizeof(int) * c->arena.nslots));
+    CK(c, cudaMemsetAsync(c->pk.d_ok, 0, sizeof(int) * c->arena.nslots, st));
+    c->pk.state = 1;
+  }
+  for (int slot : *out) c->pk.dirty[slot] = 0;
+  return B2M_OK;
+}
+
 // ---------------- cache policy ----------------
 int pick_victim(b2m_ctx* c, const std::vector<int>& in_use, bool allow_protected) {
   const int L = c->cfg.num_layers, E = c->cfg.num_experts;
@@ -529,6 +591,8 @@ int issue_copy(b2m_ctx* c, int id, int slot, cudaStream_t st, bool do_copy) {
     int r = copy_from_store(c, x, dst, st, st != c->prefetch_stream);
     if (r) { c->free_slots.push_back(slot); return r; }   // the expert stays on the store; its slot goes back
   }
+  int r = pk_invalidate(c, slot, st);
+  if (r) return r;
   if (!x.ready) CK(c, cudaEventCreateWithFlags(&x.ready, cudaEventDisableTiming));
   CK(c, cudaEventRecord(x.ready, st));
   x.ready_pending = true;
@@ -722,6 +786,11 @@ int b2m_ctx_create(const b2m_config* cfg, b2m_ctx** out) {
   c->offload = nslots < (long long)L * E;
   CKC(cudaMalloc((void**)&c->arena.base, (size_t)nslots * shape.bytes));
   c->arena.owned = true;
+  for (int m = 0; m < 3; ++m) {
+    c->pk.off[m] = c->pk.slot_bytes;
+    c->pk.slot_bytes += packed_matrix_bytes((int)pk_matrix_rows(shape, m), (int)pk_matrix_cols(shape, m));
+  }
+  c->pk.dirty.assign((size_t)nslots, PK_WRITTEN);
   const bool tc = cfg->dtype != B2M_DTYPE_F32;   // fp32 experts run on the CUDA-core path (f32_path.cu): no TMA maps
   int r = tc ? build_arena_maps(c, &c->arena) : B2M_OK;
   if (r) { g_create_error = c->err; b2m_ctx_destroy(c); return r; }
@@ -815,6 +884,8 @@ int b2m_ctx_destroy(b2m_ctx* c) {
   cudaDeviceSynchronize();
   if (c->arena.owned && c->arena.base) cudaFree(c->arena.base);
   if (c->shared_arena.owned && c->shared_arena.base) cudaFree(c->shared_arena.base);
+  if (c->pk.base) cudaFree(c->pk.base);
+  if (c->pk.d_ok) cudaFree(c->pk.d_ok);
   void* bufs[] = {c->d_slot_of, c->d_topk_idx, c->d_topk_w, c->d_row_of, c->d_perm_token, c->d_counts, c->d_offsets,
                   c->d_chunk_counts, c->d_offsets_src, c->d_ticket, c->d_gbar, c->d_err, c->d_look, c->d_tl, c->d_dest_of, c->d_scores, c->d_logits, c->d_xp, c->d_hmid, c->d_y, c->d_hmid_s, c->d_y_s};
   for (void* b : bufs) if (b) cudaFree(b);
@@ -912,7 +983,6 @@ int b2m_host_unpin(b2m_ctx* c, void* host_ptr) {
 }
 
 int b2m_make_resident(b2m_ctx* c, int layer, int expert, int flags, void* stream) {
-  (void)stream;
   int r = check_layer(c, layer);
   if (r) return r;
   if (expert < 0 || expert >= c->cfg.num_experts) return fail(c, B2M_EINVAL, "expert %d out of range", expert);
@@ -939,6 +1009,7 @@ int b2m_make_resident(b2m_ctx* c, int layer, int expert, int flags, void* stream
   }
   if (flags & 1) x.pinned = true;
   if (!x.backed()) x.pinned = true;
+  if (no_copy) return pk_invalidate(c, x.slot, (cudaStream_t)stream);   // the caller fills the slot next
   return B2M_OK;
 }
 
@@ -948,7 +1019,7 @@ int b2m_expert_dev_ptr(b2m_ctx* c, int layer, int expert, void** dev_ptr) {
   if (expert < 0 || expert >= c->cfg.num_experts || !dev_ptr) return fail(c, B2M_EINVAL, "bad argument");
   const Expert& x = c->experts[(size_t)layer * c->cfg.num_experts + expert];
   *dev_ptr = x.slot >= 0 ? c->arena.base + (size_t)x.slot * c->arena.slot_bytes : nullptr;
-  return B2M_OK;
+  return pk_invalidate(c, x.slot, 0);   // a writable view: the slot may change before the next forward
 }
 
 int b2m_shared_dev_ptr(b2m_ctx* c, int layer, void** dev_ptr) {
@@ -1019,7 +1090,7 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
   // has finished, so a GEMM that reads offsets/slot_of before its own griddepcontrol.wait could see the previous layer's
   // tables.  Pre-wait reads may only touch data older than the predecessor's own launch.
   c->k3_early_ok = k3_early && !pdl_enabled() && T >= 1 && T <= 256 && c->cfg.router != B2M_ROUTER_SWITCH_TOP1 && !ep_dispatch &&
-                   !c->offload && !c->ep_mode && c->cfg.gemm_impl == 0;
+                   !c->offload && !c->ep_mode && c->cfg.gemm_impl != 1;
   p.offsets_early = c->k3_early_ok ? 1 : 0;
   const bool rows_by_gate = sw().rows_by_gate;
   p.rows_by_gate = (c->k3_early_ok && rows_by_gate) ? 1 : 0;
@@ -1118,6 +1189,33 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
 #else
     const bool mc2 = false;
 #endif
+    // packed weights (decode-sized tiles of the routed experts); this call's gate/up launch first packs the stale slots it
+    // was handed (base.pack_slots), the down launch never packs
+    dn.pack_n = 0;
+    if (&a == &c->arena && c->pk.state == 1) {
+      up.pk_ok = dn.pk_ok = c->pk.d_ok;
+      up.pk_slot_bytes = dn.pk_slot_bytes = c->pk.slot_bytes;
+      up.pk_bit0 = 0; up.pk_bit1 = 1;
+      up.pk_a0 = c->pk.base + c->pk.off[0];
+      up.pk_a1 = c->pk.base + c->pk.off[1];
+      dn.pk_bit0 = dn.pk_bit1 = 2;
+      dn.pk_a0 = dn.pk_a1 = c->pk.base + c->pk.off[2];
+      up.pack_ok = c->pk.d_ok;
+      up.pack_dst = c->pk.base;
+      up.pack_src = a.base;
+      up.pack_src_slot_bytes = a.slot_bytes;
+      up.pack_nmat = 3;
+      const size_t src_off[3] = {s.off_gate, s.off_up, s.off_down};
+      for (int m = 0; m < 3; ++m) {
+        up.pack_src_off[m] = src_off[m];
+        up.pack_dst_off[m] = c->pk.off[m];
+        up.pack_rows[m] = (int)pk_matrix_rows(s, m);
+        up.pack_cols[m] = (int)pk_matrix_cols(s, m);
+      }
+    } else {
+      up.pack_n = 0;
+    }
+    if (up.pack_n > 0) c->stats.kernel_launches += 2;   // pack + publish flags
     const bool pdl_k3 = sw().pdl_k3;
     up.pdl_edge = (pdl_k3 && !T_hint_large) ? 1 : 0;
     up.early_a = (c->k3_early_ok && &a == &c->arena && phases == 3) ? 1 : 0;   // routed experts right behind the permute kernel
@@ -1151,7 +1249,7 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
       // decode: let the down projection start under the tail of the gate/up GEMM and prefetch its first weight tiles
       // B2M_EARLY_A=0 disables
       const bool early_a = sw().early_a;
-      dn.early_a = (early_a && !pdl_enabled() && (phases & 1) && f.gemm_impl == 0 && !T_hint_large) ? 1 : 0;
+      dn.early_a = (early_a && !pdl_enabled() && (phases & 1) && f.gemm_impl != 1 && !T_hint_large) ? 1 : 0;
       // split-K at decode: equal contiguous shares of all (tile, k-block) units per CTA instead of a fixed factor, so no
       // SM is left with an extra slice in the last wave (B2M_STREAMK=0: fixed factor)
       const bool streamk = sw().streamk;
@@ -1292,9 +1390,14 @@ int b2m_run_experts_ex(b2m_ctx* c, int layer, int T, int phases, void* stream) {
     }
     const bool whole = wave.size() == active.size();
     if (!whole && phases != 3) return fail(c, B2M_ESTATE, "phase-split launches need the whole active set resident");
+    std::vector<int> pack;
     if (whole) {
       r = upload_row_if_dirty(c, layer, st);
       if (r) return r;
+      if (phases & 1) {   // the gate/up launch packs
+        r = pk_collect(c, layer, st, &pack);
+        if (r) return r;
+      }
     } else {
       // partial wave: the device row names only this wave's experts (others -1 => their tiles are skipped)
       if (waves > 0 && waves % (STAGE_RING - 1) == 0) CK(c, cudaStreamSynchronize(st));   // staging ring would wrap
@@ -1305,7 +1408,10 @@ int b2m_run_experts_ex(b2m_ctx* c, int layer, int T, int phases, void* stream) {
       CK(c, cudaMemcpyAsync(c->d_slot_of + (size_t)layer * E, stage, sizeof(int) * E, cudaMemcpyHostToDevice, st));
       c->row_dirty[layer] = 1;   // the true mapping is re-uploaded by the next whole-wave call
     }
-    r = launch_expert_gemms(c, c->arena, base, c->tm_xp[ni], c->tm_hmid[nd], c->d_xp, c->cfg.hidden, c->d_hmid,
+    GemmParams wave_base = base;
+    wave_base.pack_slots = pack.data();
+    wave_base.pack_n = (int)pack.size();
+    r = launch_expert_gemms(c, c->arena, wave_base, c->tm_xp[ni], c->tm_hmid[nd], c->d_xp, c->cfg.hidden, c->d_hmid,
                             c->d_hmid, c->d_y, c->cur_nt, c->cur_nt_dn, c->cur_ksplit, st, phases);
     if (r) return r;
     if (on_demand) {
@@ -1813,7 +1919,7 @@ int b2m_ep_p2p_layer(b2m_ctx* c, int layer, const void* x, const void* router_in
   const int El = f.num_experts / q.nranks, R = q.nranks * q.cap, T_total = q.nranks * T_local;
   const bool direct_on = sw().ep_direct;
   // direct mode: the fused route+dispatch kernel needs every CTA resident (T_local <= #SMs)
-  const bool direct = direct_on && T_local <= c->num_sms && f.gemm_impl == 0 && f.shared_inter == 0 &&
+  const bool direct = direct_on && T_local <= c->num_sms && f.gemm_impl != 1 && f.shared_inter == 0 &&
                       f.router != B2M_ROUTER_SWITCH_TOP1 && f.dtype != B2M_DTYPE_F32;
   cudaStream_t st = (cudaStream_t)stream;
   if (!direct) {

@@ -71,7 +71,31 @@ struct GemmParams {
   int* ep_peer_done_flag[16];  // peer r's done_flag[nranks] (this rank writes entry [rank])
   int ep_rank;
   unsigned long long* tl;    // optional timeline slots of this launch: [0] first CTA start, [1] peers' flags seen, [2] last CTA end (ns)
+  // ---- packed weights (weight_pack.cuh; bf16, 16..64-token tiles, single 128-row m-tiles).  pk_ok[slot] bit b set: matrix b
+  // of the slot has a current packed copy, read instead of the bf16 arena.  A0 / A1 of this GEMM are matrices pk_bit0 / pk_bit1.
+  const int* pk_ok;          // null = bf16 only
+  int pk_bit0, pk_bit1;
+  const uint8_t* pk_a0;      // packed A0 / A1 of slot 0: records in (m-tile, k-block) order, pk_slot_bytes apart
+  const uint8_t* pk_a1;
+  size_t pk_slot_bytes;
+  // packing request (host side, read by launch_grouped_gemm_tc before it launches the GEMM): pack the matrices of these slots
+  const int* pack_slots;     // host array, pack_n entries; null / 0 = nothing to pack
+  int pack_n;
+  int pack_nmat;             // matrices per slot
+  const uint8_t* pack_src;   // bf16 arena
+  size_t pack_src_slot_bytes;
+  size_t pack_src_off[3];    // byte offset of matrix b inside a bf16 slot ...
+  size_t pack_dst_off[3];    // ... and of its packed copy inside a packed slot
+  int pack_rows[3], pack_cols[3];
+  uint8_t* pack_dst;         // packed arena (pk_slot_bytes per slot)
+  int* pack_ok;              // = pk_ok, writable
 };
+
+// packed copy of a rows x cols K-major bf16 matrix (weight_pack.cuh); 0 when its shape does not divide into tiles
+inline size_t packed_matrix_bytes(int rows, int cols) {
+  if (rows % 128 || cols % 64) return 0;
+  return (size_t)(rows / 128) * (size_t)(cols / 64) * (128 + 12288);
+}
 
 cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1,
                                    const CUtensorMap& b, const GemmParams& p, int grid, cudaStream_t st);

@@ -16,10 +16,16 @@
 //   DUAL  = gate and up projections share the token tile and are fused with act(g)*u in the epilogue.
 //   !DUAL = single projection: activation epilogue (Switch wi + ReLU) or linear fp32 output
 //           (down projection), optionally split-K with fp32 red.add.
+#include <string.h>
+
+#include <algorithm>
+#include <type_traits>
+
 #include "b2m_common.cuh"
 #include "b2m_internal.h"
 #include "ep_device.cuh"
 #include "tile_walker.cuh"
+#include "weight_pack.cuh"
 
 namespace b2m {
 
@@ -30,7 +36,7 @@ constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
 constexpr int MAX_E = 256;
 constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on sm_90; the rest holds barriers and tile tables
 
-template <int NT, bool DUAL>
+template <int NT, bool DUAL, bool PK = false>
 struct GemmCfg {
   static constexpr int B_TILE_BYTES = NT * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_TILE_BYTES + B_TILE_BYTES;
@@ -46,16 +52,18 @@ struct GemmCfg {
   // that allocation, so the producer warpgroup (one issuing lane) drops to 40 and the consumers take what it frees (a
   // request beyond the allocation would never be granted).  launch_tc checks LAUNCH_REGS against the compiled kernel.
   static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
-  static constexpr int PRODUCER_REGS = 40;
+  // (the packed-weight producer also walks record addresses: 48 keeps it free of spills)
+  static constexpr int PRODUCER_REGS = PK ? 48 : 40;
   static constexpr int CONSUMER_REGS_RAW = (LAUNCH_REGS * THREADS - 128 * PRODUCER_REGS) / (128 * CONSUMERS);
   static constexpr int CONSUMER_REGS = (CONSUMER_REGS_RAW > 240 ? 240 : CONSUMER_REGS_RAW) & ~7;
   static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 128 * CONSUMERS <= LAUNCH_REGS * THREADS, "register split too large");
   static_assert(CONSUMER_REGS >= LAUNCH_REGS, "setmaxnreg.inc must not lower the consumers' count");
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ +
-                                    (MAX_E + 1) * 4 * 2 /*tile_start, offsets*/ + MAX_E * 4 * 2 /*slots, region counts*/;
+                                    (MAX_E + 1) * 4 * 2 /*tile_start, offsets*/ + MAX_E * 4 * 3 /*slots, region counts, packed flags*/;
   static_assert(!(DUAL && NT > 128), "DUAL tiles are at most 128 tokens wide");
   static_assert(STAGES >= 2, "need >=2 stages");
   static_assert(SMEM_BYTES <= 227 * 1024, "over the sm_90 shared-memory limit");
+  static_assert(wp::REC_BYTES <= A_TILE_BYTES && wp::ROWS == BLOCK_M && wp::COLS == BLOCK_K, "a packed record fills an A slot of the stage");
 };
 
 __device__ __forceinline__ float act_apply(float x, int act) {
@@ -109,10 +117,13 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
 // Used as the whole body of grouped_gemm_tc_kernel and, twice, by fused_ffn_kernel (gate/up phase, grid barrier, down phase).
 // `ctas` = how many CTAs of the grid take tiles of this phase.  REGSPLIT: rebalance registers between producer and consumers
 // (once per kernel: the two-phase fused kernel keeps the even split).
-template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true>
+// PK (bf16, NT <= 64, MC == 1, no dual_m / m_rows / expert-parallel regions): a weight matrix whose packed copy is current
+// (p.pk_ok) streams as 12-bit records (weight_pack.cuh) with one bulk copy per (tile, k-block); the consumers decode their A
+// fragments into registers and issue register-A wgmmas.  Other matrices take the bf16 TMA path.
+template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, bool PK = false>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
                                           const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
-  using Cfg = GemmCfg<NT, DUAL>;
+  using Cfg = GemmCfg<NT, DUAL, PK>;
   // carve shared memory: [stages | barriers | tile tables]
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
@@ -122,6 +133,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   int* offs = tile_start + (MAX_E + 1);
   int* slots = offs + (MAX_E + 1);
   int* cnts = slots + MAX_E;           // direct mode: rows per expert region
+  int* pkf = cnts + MAX_E;             // PK: pk_ok of each expert's slot
+  static_assert(!PK || (MC == 1 && DT == DT_BF16 && NT <= 64), "packed weights: bf16 decode-sized tiles");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -198,6 +211,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
     for (int i = threadIdx.x; i < E; i += Cfg::THREADS) slots[i] = p.slot_of[i];
   }
   __syncthreads();
+  if constexpr (PK) {
+    for (int i = threadIdx.x; i < E; i += Cfg::THREADS) pkf[i] = slots[i] >= 0 ? p.pk_ok[slots[i]] : 0;
+    __syncthreads();
+  }
   if (threadIdx.x == 0) {
     int acc = 0;
     for (int e = 0; e < E; ++e) {
@@ -233,18 +250,29 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       bool waited = !p.early_a;
       int npend = 0, pend_stage[Cfg::STAGES], pend_kb[Cfg::STAGES], pend_row[Cfg::STAGES];
       for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
+        // packed records stream only when every A matrix of the tile has a current packed copy (the consumers decide the same)
+        const bool pk0 = PK && ((pkf[t.e] >> p.pk_bit0) & 1) && (!DUAL || ((pkf[t.e] >> p.pk_bit1) & 1));
+        // packed records of this tile's k-blocks: (m-tile, k-block) order inside the slot's copy of the matrix
+        const uint8_t* rec = pk0 ? p.pk_a0 + (size_t)t.slot * p.pk_slot_bytes + (size_t)(t.m0 / BLOCK_M) * kblocks * wp::REC_BYTES
+                                 : nullptr;
         for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sA0 = stage_base + stage * Cfg::STAGE_BYTES;
           uint8_t* sA1 = sA0 + A_TILE_BYTES;
           uint8_t* sB = sA0 + (DUAL ? 2 : 1) * A_TILE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], (DUAL ? 2 : 1) * m_rows * BLOCK_K * 2 + Cfg::B_TILE_BYTES);
+          const int a_bytes = m_rows * BLOCK_K * 2;
+          mbar_arrive_expect_tx(&full_bar[stage], (DUAL ? 2 : 1) * (pk0 ? wp::REC_BYTES : a_bytes) + Cfg::B_TILE_BYTES);
           // decode: weights are streamed exactly once -> evict-first.  Several n-tiles per expert (prefill): the same
           // weight tile is re-read by every n-tile -> keep it in L2.  Tokens are re-read by every m-tile: keep.
           const uint64_t wh = ((p.ep_rows > 0 ? cnts[t.e] : offs[t.e + 1] - offs[t.e]) <= NT) ? CACHE_EVICT_FIRST : CACHE_EVICT_NORMAL;
           if (MC == 1) {
-            tma_load_3d(&tmA0, &full_bar[stage], sA0, kb * BLOCK_K, t.m0, t.slot, wh);
-            if (DUAL) tma_load_3d(&tmA1, &full_bar[stage], sA1, kb * BLOCK_K, t.m0 + (p.dual_m ? BLOCK_M : 0), t.slot, wh);
+            if (pk0) {
+              bulk_load(&full_bar[stage], sA0, rec + (size_t)kb * wp::REC_BYTES, wp::REC_BYTES, wh);
+              if (DUAL) bulk_load(&full_bar[stage], sA1, rec + (p.pk_a1 - p.pk_a0) + (size_t)kb * wp::REC_BYTES, wp::REC_BYTES, wh);
+            } else {
+              tma_load_3d(&tmA0, &full_bar[stage], sA0, kb * BLOCK_K, t.m0, t.slot, wh);
+              if (DUAL) tma_load_3d(&tmA1, &full_bar[stage], sA1, kb * BLOCK_K, t.m0 + (p.dual_m ? BLOCK_M : 0), t.slot, wh);
+            }
           } else {
             // 2-CTA multicast: the cluster's CTAs work on the same weight tiles and adjacent token tiles; each CTA fetches
             // HALF of every weight tile (64 rows; tmA* carry 64-row boxes) and multicasts it into both CTAs' stages, so
@@ -307,9 +335,22 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       if (MC == 1) mbar_arrive(&empty_bar[s]);
       else for (int c = 0; c < MC; ++c) mbar_arrive_cluster(&empty_bar[s], (uint32_t)c);   // the peer multicasts into it too
     };
+    // PK: decoded A fragments, double-buffered -- the wgmmas of the k-block in flight still read one buffer while the next
+    // k-block is decoded into the other (wgmma_wait<1> retires the older one)
+    uint32_t fa0[2][16], fa1[2][16];   // (unused without PK)
     for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
       int prev = -1;
-      for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
+      auto next_stage = [&]() {
+        wgmma_commit();
+        wgmma_fence_regs(acc0);
+        if (DUAL) wgmma_fence_regs(acc1);
+        wgmma_wait<1>();                 // the previous k-block's wgmmas have read their operands: that stage may be refilled
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+      };
+      // one k-block, A from the bf16 tile in shared memory
+      auto kblock_smem = [&](int kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a0 = smem_u32(stage_base + stage * Cfg::STAGE_BYTES) + mh * (64 * BLOCK_K * 2);
         const uint32_t b = smem_u32(stage_base + stage * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_TILE_BYTES);
@@ -318,13 +359,40 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         wgmma_fence();
         wgmma_kblock<NT, DT>(acc0, make_kmajor_sw128_desc(a0), make_kmajor_sw128_desc(b), kb == t.kb_begin);
         if constexpr (DUAL) wgmma_kblock<NT, DT>(acc1, make_kmajor_sw128_desc(a0 + A_TILE_BYTES), make_kmajor_sw128_desc(b), kb == t.kb_begin);
-        wgmma_commit();
+        next_stage();
+      };
+      // one k-block, A decoded from packed records into fragment buffer BUF (compile time)
+      auto kblock_packed = [&](int kb, auto BUF) {
+        constexpr int bf = decltype(BUF)::value;
+        mbar_wait(&full_bar[stage], phase);
+        const uint8_t* sa = stage_base + stage * Cfg::STAGE_BYTES;
+        wp::decode_lane(sa, ct, fa0[bf]);
+        if constexpr (DUAL) wp::decode_lane(sa + A_TILE_BYTES, ct, fa1[bf]);
+        const uint64_t db = make_kmajor_sw128_desc(smem_u32(sa + (DUAL ? 2 : 1) * A_TILE_BYTES));
         wgmma_fence_regs(acc0);
         if (DUAL) wgmma_fence_regs(acc1);
-        wgmma_wait<1>();                 // the previous k-block's wgmmas have read their operands: that stage may be refilled
-        if (prev >= 0) release(prev);
-        prev = stage;
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+          const uint64_t koff = (uint64_t)((k * MMA_K * 2) >> 4);
+          const uint32_t acc = (kb != t.kb_begin || k > 0) ? 1u : 0u;
+          wgmma_rs_bf16<NT>(acc0, fa0[bf][4 * k], fa0[bf][4 * k + 1], fa0[bf][4 * k + 2], fa0[bf][4 * k + 3], db + koff, acc);
+          if constexpr (DUAL)
+            wgmma_rs_bf16<NT>(acc1, fa1[bf][4 * k], fa1[bf][4 * k + 1], fa1[bf][4 * k + 2], fa1[bf][4 * k + 3], db + koff, acc);
+        }
+        next_stage();
+      };
+      // a tile streams packed records when every A matrix it reads has a current packed copy (the producer decides the same)
+      bool packed = false;
+      if constexpr (PK) packed = ((pkf[t.e] >> p.pk_bit0) & 1) && (!DUAL || ((pkf[t.e] >> p.pk_bit1) & 1));
+      if (!packed) {
+        for (int kb = t.kb_begin; kb < t.kb_end; ++kb) kblock_smem(kb);
+      } else if constexpr (PK) {
+        for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
+          kblock_packed(kb, std::integral_constant<int, 0>{});
+          if (++kb >= t.kb_end) break;
+          kblock_packed(kb, std::integral_constant<int, 1>{});
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc0);
@@ -419,8 +487,8 @@ __device__ __forceinline__ uint8_t* smem_aligned(uint8_t* raw) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
 }
 
-template <int NT, bool DUAL, int DT, int MC>
-__global__ void __launch_bounds__((GemmCfg<NT, DUAL>::THREADS), 1)
+template <int NT, bool DUAL, int DT, int MC, bool PK>
+__global__ void __launch_bounds__((GemmCfg<NT, DUAL, PK>::THREADS), 1)
 grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                        const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -431,7 +499,7 @@ grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_co
   // counters) in ITS prologue, so it must not be released before this grid has passed its own wait: gemm_body triggers then.
   if (!p.pdl_edge) pdl_launch();
   GridBar nobar{nullptr, 0};
-  gemm_body<NT, DUAL, DT, MC>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
+  gemm_body<NT, DUAL, DT, MC, true, PK>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
   gemm_finish<MC>(p);
 }
 
@@ -540,11 +608,11 @@ __global__ void grouped_gemm_simt_kernel(const uint16_t* __restrict__ arena, siz
 // --------------------------------------------------------------------------------------
 // host launchers
 // --------------------------------------------------------------------------------------
-template <int NT, bool DUAL, int DT, int MC = 1>
+template <int NT, bool DUAL, int DT, int MC = 1, bool PK = false>
 static cudaError_t launch_tc(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmParams& p,
                              int grid, cudaStream_t st) {
-  using Cfg = GemmCfg<NT, DUAL>;
-  auto kern = grouped_gemm_tc_kernel<NT, DUAL, DT, MC>;
+  using Cfg = GemmCfg<NT, DUAL, PK>;
+  auto kern = grouped_gemm_tc_kernel<NT, DUAL, DT, MC, PK>;
   static bool attr_done = false;   // per-instantiation
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -606,6 +674,20 @@ cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& g, const CUte
 template <int DT>
 static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
                                const GemmParams& p, int grid, cudaStream_t st) {
+  // packed weights: decode-sized tiles only (at prefill the GEMM is tensor-bound and keeps the shared-memory A operand)
+  if constexpr (DT == DT_BF16) {
+    if (p.pk_ok && nt <= 64 && !p.dual_m && p.m_rows == 0 && p.ep_rows == 0) {
+#define B2M_PCASE(N)                                                                \
+  case N:                                                                           \
+    return dual ? launch_tc<N, true, DT, 1, true>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, true>(a0, a1, b, p, grid, st);
+      switch (nt) {
+        B2M_PCASE(16)
+        B2M_PCASE(32)
+        B2M_PCASE(64)
+      }
+#undef B2M_PCASE
+    }
+  }
 #define B2M_CASE(N)                                                                 \
   case N:                                                                           \
     return dual ? launch_tc<N, true, DT>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT>(a0, a1, b, p, grid, st);
@@ -636,9 +718,143 @@ cudaError_t launch_grouped_gemm_tc_mc2(int dtype, bool dual, const CUtensorMap& 
 }
 #endif
 
+// --------------------------------------------------------------------------------------
+// packing: bf16 slot arena -> 12-bit packed copy (weight_pack.cuh).  One CTA of LANES threads codes one tile at a time, thread L
+// the values of consumer lane L; a tile that cannot be coded marks its matrix bad (pk_ok bit 8 + matrix), and the finish kernel
+// then publishes pk_ok[slot] = the matrices whose every tile was coded.
+// --------------------------------------------------------------------------------------
+struct PackArgs {
+  const uint8_t* src;
+  size_t src_slot_bytes;
+  uint8_t* dst;
+  size_t dst_slot_bytes;
+  size_t src_off[3], dst_off[3];
+  int cols[3], kblocks[3];
+  long long tiles_before[4];   // prefix sums of the tiles of matrices 0..2 of one slot
+  int* ok;
+  int n;
+  int slots[MAX_E];
+};
+
+__global__ void __launch_bounds__(wp::LANES) pack_weights_kernel(const __grid_constant__ PackArgs a) {
+  __shared__ int s_max, s_special, s_np;
+  __shared__ uint32_t s_patch[wp::MAX_PATCH];
+  const int L = threadIdx.x;
+  const long long per_slot = a.tiles_before[3];
+  for (long long tile = blockIdx.x; tile < per_slot * a.n; tile += gridDim.x) {
+    const int slot = a.slots[tile / per_slot];
+    long long r = tile % per_slot;
+    const int m = r < a.tiles_before[1] ? 0 : r < a.tiles_before[2] ? 1 : 2;
+    r -= a.tiles_before[m];
+    const int mt = (int)(r / a.kblocks[m]), kb = (int)(r % a.kblocks[m]);
+    const uint16_t* src = reinterpret_cast<const uint16_t*>(a.src + (size_t)slot * a.src_slot_bytes + a.src_off[m]) +
+                          (size_t)mt * wp::ROWS * a.cols[m] + (size_t)kb * wp::COLS;
+    uint8_t* rec = a.dst + (size_t)slot * a.dst_slot_bytes + a.dst_off[m] + (size_t)r * wp::REC_BYTES;
+    if (L == 0) { s_max = 0; s_special = 0; s_np = 0; }
+    uint16_t u[wp::VALS];
+    int me = 0;
+    bool special = false;
+#pragma unroll
+    for (int v = 0; v < wp::VALS; v += 2) {   // values v, v + 1 are adjacent columns of one row
+      int row, col;
+      wp::lane_coord(L, v, &row, &col);
+      const uint32_t two = *reinterpret_cast<const uint32_t*>(src + (size_t)row * a.cols[m] + col);
+      u[v] = (uint16_t)two;
+      u[v + 1] = (uint16_t)(two >> 16);
+    }
+#pragma unroll
+    for (int v = 0; v < wp::VALS; ++v) {
+      const int e = wp::bf16_exp(u[v]);
+      special |= e == 255;
+      me = e > me ? e : me;
+    }
+    me = __reduce_max_sync(0xffffffffu, me);
+    special = __any_sync(0xffffffffu, special);
+    __syncthreads();
+    if ((L & 31) == 0) {
+      atomicMax(&s_max, me);
+      if (special) s_special = 1;
+    }
+    __syncthreads();
+    const int base = wp::window_base(s_max);
+    uint16_t pre[wp::VALS];
+#pragma unroll
+    for (int v = 0; v < wp::VALS; ++v)
+      if (!wp::to_pre(u[v], base, &pre[v])) {
+        const int i = atomicAdd(&s_np, 1);
+        if (i < wp::MAX_PATCH) s_patch[i] = (uint32_t)(L * wp::VALS + v) | ((uint32_t)u[v] << 16);
+      }
+    __syncthreads();
+    const int np = s_np;
+    const bool ok = !s_special && base <= wp::MAX_BASE && np <= wp::MAX_PATCH;
+    if (ok) {
+      uint32_t w[12];
+      wp::pack_lane(pre, w);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        *reinterpret_cast<uint4*>(rec + wp::body_word_offset(L, 4 * c)) = make_uint4(w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]);
+    }
+    if (L < wp::HDR_BYTES / 4) {
+      const int i = L - 4;
+      const uint32_t hw = L == 0 ? wp::header_word0(ok ? base : 0, ok ? np : 0, !ok) : (ok && i >= 0 && i < np) ? s_patch[i] : 0u;
+      reinterpret_cast<uint32_t*>(rec)[L] = hw;
+    }
+    if (!ok && L == 0) atomicOr(a.ok + slot, 1 << (8 + m));
+    __syncthreads();   // the tile's shared state is reset by the next iteration
+  }
+}
+
+__global__ void pack_finish_kernel(const __grid_constant__ PackArgs a, int mats) {
+  for (int i = threadIdx.x; i < a.n; i += blockDim.x) {
+    int* f = a.ok + a.slots[i];
+    *f = mats & ~(*f >> 8);
+  }
+}
+
+static cudaError_t launch_pack(const GemmParams& p, cudaStream_t st) {
+  if (p.pack_n > MAX_E || !p.pack_ok || !p.pack_dst || !p.pack_src) return cudaErrorInvalidValue;
+  PackArgs a;
+  memset(&a, 0, sizeof a);
+  a.src = p.pack_src;
+  a.src_slot_bytes = p.pack_src_slot_bytes;
+  a.dst = p.pack_dst;
+  a.dst_slot_bytes = p.pk_slot_bytes;
+  a.ok = p.pack_ok;
+  a.n = p.pack_n;
+  int mats = 0;
+  for (int m = 0; m < 3; ++m) {
+    const int rows = m < p.pack_nmat ? p.pack_rows[m] : 0, cols = m < p.pack_nmat ? p.pack_cols[m] : 0;
+    const bool on = packed_matrix_bytes(rows, cols) > 0 && rows > 0;
+    a.src_off[m] = p.pack_src_off[m];
+    a.dst_off[m] = p.pack_dst_off[m];
+    a.cols[m] = cols;
+    a.kblocks[m] = on ? cols / wp::COLS : 1;
+    a.tiles_before[m + 1] = a.tiles_before[m] + (on ? (long long)(rows / wp::ROWS) * (cols / wp::COLS) : 0);
+    if (on) mats |= 1 << m;
+  }
+  for (int i = 0; i < p.pack_n; ++i) a.slots[i] = p.pack_slots[i];
+  const long long tiles = a.tiles_before[3] * a.n;
+  if (tiles == 0) return cudaSuccess;
+  pack_weights_kernel<<<(unsigned)std::min<long long>(tiles, (long long)H100_SMS * 8), wp::LANES, 0, st>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  pack_finish_kernel<<<1, 256, 0, st>>>(a, mats);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1,
                                    const CUtensorMap& b, const GemmParams& p, int grid, cudaStream_t st) {
   if (p.E > MAX_E) return cudaErrorInvalidValue;
+  if (p.pack_n > 0) {
+    // pack first, then run this GEMM as a plain stream-ordered launch: its prologue reads the flags the packing just wrote
+    cudaError_t e = launch_pack(p, st);
+    if (e != cudaSuccess) return e;
+    GemmParams q = p;
+    q.pack_n = 0;
+    q.early_a = 0;
+    q.pdl_edge = 0;
+    return launch_grouped_gemm_tc(dtype, nt, dual, a0, a1, b, q, grid, st);
+  }
   if (dtype == DT_BF16) return dispatch_nt<DT_BF16>(nt, dual, a0, a1, b, p, grid, st);
   if (dtype == DT_F16) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
   return cudaErrorInvalidValue;

@@ -46,7 +46,8 @@ class MoEEngine:
                  topk_group: int = 1, norm_topk_prob: bool = False, routed_scaling_factor: float = 1.0,
                  expert_capacity: int = 0, gate_dtype: Optional[torch.dtype] = None, device: int = 0,
                  max_inflight_prefetch: int = 2, h2d_chunk_bytes: int = 0, gemm_impl: int = 0,
-                 cache_policy: int = L.CACHE_REFERENCE, lookahead_prefetch: bool = False, freq_alpha: float = 0.0):
+                 cache_policy: int = L.CACHE_REFERENCE, lookahead_prefetch: bool = False, freq_alpha: float = 0.0,
+                 pack_weights: bool = True):
         self.lib = L.load()
         if not torch.cuda.is_available():
             raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -74,7 +75,8 @@ class MoEEngine:
         cfg.device_memory_ratio = device_memory_ratio
         cfg.max_inflight_prefetch = max_inflight_prefetch
         cfg.h2d_chunk_bytes = h2d_chunk_bytes
-        cfg.gemm_impl = gemm_impl
+        # gemm_impl 2: tensor cores without the packed copy of the experts (see include/b2m.h)
+        cfg.gemm_impl = 2 if (gemm_impl == 0 and not pack_weights) else gemm_impl
         cfg.cache_policy = cache_policy
         cfg.lookahead_prefetch = int(lookahead_prefetch)
         cfg.freq_alpha = freq_alpha
@@ -153,7 +155,9 @@ class MoEEngine:
 
     def load_expert(self, layer: int, expert: int, tensors: Optional[Sequence[torch.Tensor]] = None):
         """HBM-only expert: claims a slot, pins it, fills it from `tensors` (any device) if given.
-        Returns the flat device view of the slot so callers can initialise it in place."""
+        Returns the flat device view of the slot so callers can initialise it in place.  Writes through the view must be
+        issued (on the current stream) before the next forward of this layer; the second eager forward after the load packs
+        the slot for the decode GEMMs (pack_weights=True); to change the weights later, call load_expert again and write through the view it returns."""
         self._ck(self.lib.b2m_make_resident(self._h, layer, expert, 1 | 2, C.c_void_p(_stream_ptr())))
         v = self.expert_device_view(layer, expert)
         if tensors is not None:
