@@ -40,7 +40,8 @@ extern "C" {
 #define B2M_DTYPE_BF16 0
 #define B2M_DTYPE_F32 1
 #define B2M_DTYPE_F16 2
-#define B2M_DTYPE_FP8_E4M3 3 /* not supported: B2M_EUNSUPPORTED */
+#define B2M_DTYPE_FP8_E4M3 3 /* not supported as a model dtype (B2M_EUNSUPPORTED): fp8 experts are a weight format of a
+                                bf16 context, B2M_WEIGHTS_FP8_E4M3_B128 of b2m_ctx_create_ex */
 
 /* expert-type ints == reference core/parallel/expert_module.h:13-18 */
 #define B2M_EXPERT_SWITCH_DENSE_ACT_DENSE 0       /* wi, wo; ReLU            (expert_module.cpp:24-35)  */
@@ -146,6 +147,28 @@ int b2m_version(void);
  * core/parallel/expert_dispatcher.cpp:22-109) */
 int b2m_ctx_create(const b2m_config* cfg, b2m_ctx** out);
 int b2m_ctx_destroy(b2m_ctx* ctx);
+
+/* Storage format of the routed experts' weights (b2m_ctx_create_ex) */
+#define B2M_WEIGHTS_MODEL_DTYPE 0   /* cfg.dtype, as b2m_ctx_create */
+#define B2M_WEIGHTS_FP8_E4M3_B128 1 /* FP8 E4M3 matrices with one fp32 scale per 128x128 block (DeepSeek-V3 / Qwen3-MoE FP8
+                                       checkpoints).  Each routed matrix (nn.Linear [out,in], row-major) is float8_e4m3fn with
+                                       a row-major fp32 scale grid s[out/128][in/128]; the scale multiplies.  The experts
+                                       compute exactly what the bf16 engine computes on
+                                         W[r][c] = bf16(fp32(w_q[r][c]) * s[r/128][c/128])
+                                       -- one fp32 multiply rounded to nearest-even, then one rounding to bf16 (torch:
+                                       `(w_q.float() * s_expanded).to(torch.bfloat16)`); the GEMMs dequantise inside the
+                                       kernel, so results are bit-identical to a bf16 context holding those W.
+                                       Expert blob (b2m_register_expert, b2m_expert_dev_ptr): the three e4m3 matrices in the
+                                       model's tensor order (Mixtral w1|w2|w3, DeepSeek gate|up|down), then their three scale
+                                       grids in the same order, zero-padded to a multiple of 16 bytes (b2m_stats.slot_bytes).
+                                       Activations, outputs, workspaces and the router stay bf16; DeepSeek shared experts
+                                       stay bf16 (b2m_register_shared is unchanged).  Restrictions, each refused by
+                                       b2m_ctx_create_ex with B2M_EUNSUPPORTED and a message: cfg.dtype bf16; expert types
+                                       Mixtral (4) and DeepSeek (5); hidden and inter multiples of 128; gemm_impl 0 or 2 (the
+                                       12-bit packed copy of gemm_impl 0 is never made).  The expert-parallel entry points
+                                       return B2M_EUNSUPPORTED on such a context. */
+/* b2m_ctx_create with the routed experts stored in `weight_format` (B2M_WEIGHTS_*; any other value: B2M_EINVAL) */
+int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out);
 
 /* replaces: prefetch_handle.offload/register + set_topology for an expert stage + expert_dispatcher.register_expert
  * (core/parallel/expert_dispatcher.cpp:160-173; blob layout core/model/model_topology.cpp:429-431:

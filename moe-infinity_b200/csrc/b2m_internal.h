@@ -89,6 +89,11 @@ struct GemmParams {
   int pack_rows[3], pack_cols[3];
   uint8_t* pack_dst;         // packed arena (pk_slot_bytes per slot)
   int* pack_ok;              // = pk_ok, writable
+  // ---- fp8 weights (fp8_weights.cuh; bf16 activations): non-null = the A maps are uint8 maps over e4m3 matrices and
+  // f8_s0 / f8_s1 are the fp32 block-scale grids [M / 128][K / 128] of A0 / A1 in slot 0, f8_slot_bytes apart
+  const uint8_t* f8_s0;
+  const uint8_t* f8_s1;
+  size_t f8_slot_bytes;
 };
 
 // packed copy of a rows x cols K-major bf16 matrix (weight_pack.cuh); 0 when its shape does not divide into tiles

@@ -25,6 +25,7 @@
 #include "b2m_internal.h"
 #include "ep_device.cuh"
 #include "tile_walker.cuh"
+#include "fp8_weights.cuh"
 #include "weight_pack.cuh"
 
 namespace b2m {
@@ -36,10 +37,16 @@ constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
 constexpr int MAX_E = 256;
 constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on sm_90; the rest holds barriers and tile tables
 
-template <int NT, bool DUAL, bool PK = false>
+// Where a GEMM's A operand (the weight tile) comes from
+enum : int { AS_BF16 = 0,   // bf16 tile in shared memory, read by the wgmma itself
+             AS_PK12 = 1,   // bf16 tile or 12-bit packed record (weight_pack.cuh), decoded into register fragments
+             AS_FP8 = 2 };  // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
+
+template <int NT, bool DUAL, int AS = AS_BF16>
 struct GemmCfg {
+  static constexpr int A_BYTES = AS == AS_FP8 ? f8::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
   static constexpr int B_TILE_BYTES = NT * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_TILE_BYTES + B_TILE_BYTES;
+  static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_BYTES + B_TILE_BYTES;
   static constexpr int STAGES_RAW = SMEM_BUDGET / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 10 ? 10 : STAGES_RAW;
   // a consumer warpgroup holds a 64 x NT fp32 accumulator (NT/2 registers per thread, twice for DUAL): a DUAL 256-token
@@ -53,7 +60,7 @@ struct GemmCfg {
   // request beyond the allocation would never be granted).  launch_tc checks LAUNCH_REGS against the compiled kernel.
   static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;
   // (the packed-weight producer also walks record addresses: 48 keeps it free of spills)
-  static constexpr int PRODUCER_REGS = PK ? 48 : 40;
+  static constexpr int PRODUCER_REGS = AS == AS_PK12 ? 48 : 40;
   static constexpr int CONSUMER_REGS_RAW = (LAUNCH_REGS * THREADS - 128 * PRODUCER_REGS) / (128 * CONSUMERS);
   static constexpr int CONSUMER_REGS = (CONSUMER_REGS_RAW > 240 ? 240 : CONSUMER_REGS_RAW) & ~7;
   static_assert(PRODUCER_REGS * 128 + CONSUMER_REGS * 128 * CONSUMERS <= LAUNCH_REGS * THREADS, "register split too large");
@@ -64,6 +71,7 @@ struct GemmCfg {
   static_assert(STAGES >= 2, "need >=2 stages");
   static_assert(SMEM_BYTES <= 227 * 1024, "over the sm_90 shared-memory limit");
   static_assert(wp::REC_BYTES <= A_TILE_BYTES && wp::ROWS == BLOCK_M && wp::COLS == BLOCK_K, "a packed record fills an A slot of the stage");
+  static_assert(f8::ROWS == BLOCK_M && f8::COLS == BLOCK_K && A_BYTES % 1024 == 0, "an fp8 tile keeps the stage's 1024-B alignment");
 };
 
 __device__ __forceinline__ float act_apply(float x, int act) {
@@ -120,10 +128,15 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
 // PK (bf16, NT <= 64, MC == 1, no dual_m / m_rows / expert-parallel regions): a weight matrix whose packed copy is current
 // (p.pk_ok) streams as 12-bit records (weight_pack.cuh) with one bulk copy per (tile, k-block); the consumers decode their A
 // fragments into registers and issue register-A wgmmas.  Other matrices take the bf16 TMA path.
-template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, bool PK = false>
+// FP8 (AS_FP8: bf16, MC == 1, no m_rows / expert-parallel regions; every tile width): the A maps are uint8 maps over e4m3
+// matrices; the producer loads 8-KiB e4m3 tiles and the consumers dequantise their fragments with the tile's block scale
+// (fp8_weights.cuh) into the same register-A wgmmas, over the same tile walk and launch plan as the bf16 engine.
+template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, int AS = AS_BF16>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
                                           const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
-  using Cfg = GemmCfg<NT, DUAL, PK>;
+  using Cfg = GemmCfg<NT, DUAL, AS>;
+  constexpr bool PK = AS == AS_PK12, F8 = AS == AS_FP8;
+  constexpr int A_BYTES = Cfg::A_BYTES;
   // carve shared memory: [stages | barriers | tile tables]
   uint8_t* stage_base = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
@@ -135,6 +148,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   int* cnts = slots + MAX_E;           // direct mode: rows per expert region
   int* pkf = cnts + MAX_E;             // PK: pk_ok of each expert's slot
   static_assert(!PK || (MC == 1 && DT == DT_BF16 && NT <= 64), "packed weights: bf16 decode-sized tiles");
+  static_assert(!F8 || (MC == 1 && DT == DT_BF16), "fp8 weights: bf16 activations, single-CTA tiles");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -258,9 +272,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sA0 = stage_base + stage * Cfg::STAGE_BYTES;
-          uint8_t* sA1 = sA0 + A_TILE_BYTES;
-          uint8_t* sB = sA0 + (DUAL ? 2 : 1) * A_TILE_BYTES;
-          const int a_bytes = m_rows * BLOCK_K * 2;
+          uint8_t* sA1 = sA0 + A_BYTES;
+          uint8_t* sB = sA0 + (DUAL ? 2 : 1) * A_BYTES;
+          const int a_bytes = m_rows * BLOCK_K * (F8 ? 1 : 2);
           mbar_arrive_expect_tx(&full_bar[stage], (DUAL ? 2 : 1) * (pk0 ? wp::REC_BYTES : a_bytes) + Cfg::B_TILE_BYTES);
           // decode: weights are streamed exactly once -> evict-first.  Several n-tiles per expert (prefill): the same
           // weight tile is re-read by every n-tile -> keep it in L2.  Tokens are re-read by every m-tile: keep.
@@ -291,7 +305,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
             if (++npend == Cfg::STAGES) {
               if (dep_mode == DEP_PDL) pdl_wait(); else { grid_bar_wait(gbar); fence_proxy_async_global(); }
               for (int i = 0; i < npend; ++i)
-                tma_load_2d(&tmB, &full_bar[pend_stage[i]], stage_base + pend_stage[i] * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_TILE_BYTES,
+                tma_load_2d(&tmB, &full_bar[pend_stage[i]], stage_base + pend_stage[i] * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_BYTES,
                             pend_kb[i] * BLOCK_K, pend_row[i], CACHE_EVICT_LAST);
               waited = true;
             }
@@ -304,7 +318,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       if (!waited) {   // fewer work items than pipeline stages
         if (dep_mode == DEP_PDL) pdl_wait(); else { grid_bar_wait(gbar); fence_proxy_async_global(); }
         for (int i = 0; i < npend; ++i)
-          tma_load_2d(&tmB, &full_bar[pend_stage[i]], stage_base + pend_stage[i] * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_TILE_BYTES,
+          tma_load_2d(&tmB, &full_bar[pend_stage[i]], stage_base + pend_stage[i] * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_BYTES,
                       pend_kb[i] * BLOCK_K, pend_row[i], CACHE_EVICT_LAST);
       }
     }
@@ -335,9 +349,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       if (MC == 1) mbar_arrive(&empty_bar[s]);
       else for (int c = 0; c < MC; ++c) mbar_arrive_cluster(&empty_bar[s], (uint32_t)c);   // the peer multicasts into it too
     };
-    // PK: decoded A fragments, double-buffered -- the wgmmas of the k-block in flight still read one buffer while the next
-    // k-block is decoded into the other (wgmma_wait<1> retires the older one)
-    uint32_t fa0[2][16], fa1[2][16];   // (unused without PK)
+    // PK / F8: decoded A fragments, double-buffered -- the wgmmas of the k-block in flight still read one buffer while the next
+    // k-block is decoded into the other (wgmma_wait<1> retires the older one).  The fp8 DUAL 128-token tile keeps ONE buffer:
+    // beside its 128 accumulator registers a second one spills.  Its decode then waits for the previous k-block's wgmmas; the
+    // other consumer warpgroup's wgmmas keep the tensor cores busy meanwhile (this width only runs at prefill).
+    constexpr int FRAG_BUFS = (F8 && DUAL && NT == 128) ? 1 : 2;
+    uint32_t fa0[FRAG_BUFS][16], fa1[FRAG_BUFS][16];   // (unused without PK / F8)
     for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
       int prev = -1;
       auto next_stage = [&]() {
@@ -353,22 +370,52 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       auto kblock_smem = [&](int kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a0 = smem_u32(stage_base + stage * Cfg::STAGE_BYTES) + mh * (64 * BLOCK_K * 2);
-        const uint32_t b = smem_u32(stage_base + stage * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_TILE_BYTES);
+        const uint32_t b = smem_u32(stage_base + stage * Cfg::STAGE_BYTES + (DUAL ? 2 : 1) * A_BYTES);
         wgmma_fence_regs(acc0);
         if (DUAL) wgmma_fence_regs(acc1);
         wgmma_fence();
         wgmma_kblock<NT, DT>(acc0, make_kmajor_sw128_desc(a0), make_kmajor_sw128_desc(b), kb == t.kb_begin);
-        if constexpr (DUAL) wgmma_kblock<NT, DT>(acc1, make_kmajor_sw128_desc(a0 + A_TILE_BYTES), make_kmajor_sw128_desc(b), kb == t.kb_begin);
+        if constexpr (DUAL) wgmma_kblock<NT, DT>(acc1, make_kmajor_sw128_desc(a0 + A_BYTES), make_kmajor_sw128_desc(b), kb == t.kb_begin);
         next_stage();
       };
-      // one k-block, A decoded from packed records into fragment buffer BUF (compile time)
+      // FP8: block scales of this tile's A0 / A1 rows (dual_m: A1 is the next 128-row tile of the same matrix, clamped to the
+      // matrix -- a tile past its end holds TMA's zero fill and its rows are dropped).  One fp32 per 128 k, loaded one k-block
+      // ahead of its use.
+      const float* sc0 = nullptr;
+      const float* sc1 = nullptr;
+      float sn0 = 0.f, sn1 = 0.f;
+      if constexpr (F8) {
+        const int kbs = p.K / f8::BLOCK, mt = t.m0 / BLOCK_M, mts = p.M / BLOCK_M;
+        sc0 = reinterpret_cast<const float*>(p.f8_s0 + (size_t)t.slot * p.f8_slot_bytes) + (size_t)mt * kbs;
+        sc1 = DUAL ? reinterpret_cast<const float*>(p.f8_s1 + (size_t)t.slot * p.f8_slot_bytes) +
+                         (size_t)(p.dual_m && mt + 1 < mts ? mt + 1 : mt) * kbs
+                   : sc0;
+        sn0 = __ldg(sc0 + t.kb_begin / 2);
+        if (DUAL) sn1 = __ldg(sc1 + t.kb_begin / 2);
+      }
+      // one k-block, A decoded from packed records / dequantised from e4m3 into fragment buffer BUF (compile time)
       auto kblock_packed = [&](int kb, auto BUF) {
         constexpr int bf = decltype(BUF)::value;
+        float s0 = 0.f, s1 = 0.f;
+        if constexpr (F8) {
+          s0 = sn0;
+          s1 = sn1;
+          if (kb + 1 < t.kb_end) {
+            sn0 = __ldg(sc0 + (kb + 1) / 2);
+            if (DUAL) sn1 = __ldg(sc1 + (kb + 1) / 2);
+          }
+        }
         mbar_wait(&full_bar[stage], phase);
+        if constexpr (FRAG_BUFS == 1) wgmma_wait<0>();   // the previous k-block's wgmmas have read the fragments
         const uint8_t* sa = stage_base + stage * Cfg::STAGE_BYTES;
-        wp::decode_lane(sa, ct, fa0[bf]);
-        if constexpr (DUAL) wp::decode_lane(sa + A_TILE_BYTES, ct, fa1[bf]);
-        const uint64_t db = make_kmajor_sw128_desc(smem_u32(sa + (DUAL ? 2 : 1) * A_TILE_BYTES));
+        if constexpr (F8) {
+          f8::decode_lane(sa, ct, s0, fa0[bf]);
+          if constexpr (DUAL) f8::decode_lane(sa + A_BYTES, ct, s1, fa1[bf]);
+        } else {
+          wp::decode_lane(sa, ct, fa0[bf]);
+          if constexpr (DUAL) wp::decode_lane(sa + A_BYTES, ct, fa1[bf]);
+        }
+        const uint64_t db = make_kmajor_sw128_desc(smem_u32(sa + (DUAL ? 2 : 1) * A_BYTES));
         wgmma_fence_regs(acc0);
         if (DUAL) wgmma_fence_regs(acc1);
         wgmma_fence();
@@ -383,15 +430,16 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         next_stage();
       };
       // a tile streams packed records when every A matrix it reads has a current packed copy (the producer decides the same)
-      bool packed = false;
+      bool packed = F8;
       if constexpr (PK) packed = ((pkf[t.e] >> p.pk_bit0) & 1) && (!DUAL || ((pkf[t.e] >> p.pk_bit1) & 1));
       if (!packed) {
-        for (int kb = t.kb_begin; kb < t.kb_end; ++kb) kblock_smem(kb);
-      } else if constexpr (PK) {
+        if constexpr (!F8)
+          for (int kb = t.kb_begin; kb < t.kb_end; ++kb) kblock_smem(kb);
+      } else if constexpr (PK || F8) {
         for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
           kblock_packed(kb, std::integral_constant<int, 0>{});
           if (++kb >= t.kb_end) break;
-          kblock_packed(kb, std::integral_constant<int, 1>{});
+          kblock_packed(kb, std::integral_constant<int, FRAG_BUFS - 1>{});
         }
       }
       wgmma_wait<0>();
@@ -487,8 +535,8 @@ __device__ __forceinline__ uint8_t* smem_aligned(uint8_t* raw) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
 }
 
-template <int NT, bool DUAL, int DT, int MC, bool PK>
-__global__ void __launch_bounds__((GemmCfg<NT, DUAL, PK>::THREADS), 1)
+template <int NT, bool DUAL, int DT, int MC, int AS>
+__global__ void __launch_bounds__((GemmCfg<NT, DUAL, AS>::THREADS), 1)
 grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                        const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -499,7 +547,7 @@ grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_co
   // counters) in ITS prologue, so it must not be released before this grid has passed its own wait: gemm_body triggers then.
   if (!p.pdl_edge) pdl_launch();
   GridBar nobar{nullptr, 0};
-  gemm_body<NT, DUAL, DT, MC, true, PK>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
+  gemm_body<NT, DUAL, DT, MC, true, AS>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
   gemm_finish<MC>(p);
 }
 
@@ -608,11 +656,11 @@ __global__ void grouped_gemm_simt_kernel(const uint16_t* __restrict__ arena, siz
 // --------------------------------------------------------------------------------------
 // host launchers
 // --------------------------------------------------------------------------------------
-template <int NT, bool DUAL, int DT, int MC = 1, bool PK = false>
+template <int NT, bool DUAL, int DT, int MC = 1, int AS = AS_BF16>
 static cudaError_t launch_tc(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmParams& p,
                              int grid, cudaStream_t st) {
-  using Cfg = GemmCfg<NT, DUAL, PK>;
-  auto kern = grouped_gemm_tc_kernel<NT, DUAL, DT, MC, PK>;
+  using Cfg = GemmCfg<NT, DUAL, AS>;
+  auto kern = grouped_gemm_tc_kernel<NT, DUAL, DT, MC, AS>;
   static bool attr_done = false;   // per-instantiation
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -674,12 +722,31 @@ cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& g, const CUte
 template <int DT>
 static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
                                const GemmParams& p, int grid, cudaStream_t st) {
+  // fp8 weights: every tile width the bf16 plan picks, same plan (the caller's p)
+  if constexpr (DT == DT_BF16) {
+    if (p.f8_s0) {
+#define B2M_FCASE(N)                                                                \
+  case N:                                                                           \
+    return dual ? launch_tc<N, true, DT, 1, AS_FP8>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_FP8>(a0, a1, b, p, grid, st);
+      switch (nt) {
+        B2M_FCASE(16)
+        B2M_FCASE(32)
+        B2M_FCASE(64)
+        B2M_FCASE(128)
+        case 256:
+          return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_FP8>(a0, a1, b, p, grid, st);
+        default:
+          return cudaErrorInvalidValue;
+      }
+#undef B2M_FCASE
+    }
+  }
   // packed weights: decode-sized tiles only (at prefill the GEMM is tensor-bound and keeps the shared-memory A operand)
   if constexpr (DT == DT_BF16) {
     if (p.pk_ok && nt <= 64 && !p.dual_m && p.m_rows == 0 && p.ep_rows == 0) {
 #define B2M_PCASE(N)                                                                \
   case N:                                                                           \
-    return dual ? launch_tc<N, true, DT, 1, true>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, true>(a0, a1, b, p, grid, st);
+    return dual ? launch_tc<N, true, DT, 1, AS_PK12>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_PK12>(a0, a1, b, p, grid, st);
       switch (nt) {
         B2M_PCASE(16)
         B2M_PCASE(32)
@@ -856,7 +923,7 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
     return launch_grouped_gemm_tc(dtype, nt, dual, a0, a1, b, q, grid, st);
   }
   if (dtype == DT_BF16) return dispatch_nt<DT_BF16>(nt, dual, a0, a1, b, p, grid, st);
-  if (dtype == DT_F16) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
+  if (dtype == DT_F16 && !p.f8_s0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
   return cudaErrorInvalidValue;
 }
 

@@ -17,6 +17,7 @@ EXPERT_SWITCH, EXPERT_SWITCH_GATED, EXPERT_NLLB, EXPERT_FSGPT, EXPERT_MIXTRAL, E
 ROUTER_MIXTRAL, ROUTER_DEEPSEEK_GREEDY, ROUTER_DEEPSEEK_GROUP, ROUTER_SWITCH_TOP1 = 0, 1, 2, 3
 NUMERICS_REFERENCE, NUMERICS_FP32 = 0, 1
 CACHE_REFERENCE, CACHE_SLOTS, CACHE_ACTIVATION_AWARE = 0, 1, 2
+WEIGHTS_MODEL_DTYPE, WEIGHTS_FP8_E4M3_B128 = 0, 1
 WS = dict(topk_idx=0, topk_w=1, row_of=2, perm_token=3, counts=4, offsets=5, xp=6, hmid=7, y=8, scores=9, logits=10)
 
 
@@ -48,6 +49,7 @@ SYMBOLS = [
     ("b2m_last_error", C.c_char_p, [_VP]),
     ("b2m_version", _I, []),
     ("b2m_ctx_create", _I, [C.POINTER(Config), C.POINTER(_VP)]),
+    ("b2m_ctx_create_ex", _I, [C.POINTER(Config), _I, C.POINTER(_VP)]),
     ("b2m_ctx_destroy", _I, [_VP]),
     ("b2m_register_expert", _I, [_VP, _I, _I, _VP, _SZ]),
     ("b2m_register_shared", _I, [_VP, _I, _VP, _SZ]),

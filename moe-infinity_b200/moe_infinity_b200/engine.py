@@ -13,6 +13,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import torch
 
 from . import _lib as L
+from . import fp8 as F8
 
 _TORCH2INT = {torch.bfloat16: L.DTYPE_BF16, torch.float32: L.DTYPE_F32, torch.float16: L.DTYPE_F16}
 _INT2TORCH = {v: k for k, v in _TORCH2INT.items()}
@@ -47,12 +48,20 @@ class MoEEngine:
                  expert_capacity: int = 0, gate_dtype: Optional[torch.dtype] = None, device: int = 0,
                  max_inflight_prefetch: int = 2, h2d_chunk_bytes: int = 0, gemm_impl: int = 0,
                  cache_policy: int = L.CACHE_REFERENCE, lookahead_prefetch: bool = False, freq_alpha: float = 0.0,
-                 pack_weights: bool = True):
+                 pack_weights: bool = True, expert_dtype: Optional[torch.dtype] = None):
+        """expert_dtype: None = the routed experts are stored in `dtype`; torch.float8_e4m3fn = FP8 E4M3 with one fp32 scale
+        per 128x128 block (`fp8.py`; `dtype` stays the activation dtype and must be bf16; register_expert / load_expert then
+        take the three e4m3 matrices and their scale grids)."""
         self.lib = L.load()
         if not torch.cuda.is_available():
             raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if dtype not in _TORCH2INT:
             raise ValueError(f"unsupported dtype {dtype}")
+        if expert_dtype is not None and expert_dtype != torch.float8_e4m3fn:
+            raise ValueError(f"unsupported expert_dtype {expert_dtype} (None or torch.float8_e4m3fn)")
+        self.fp8 = expert_dtype is not None
+        if self.fp8 and dtype != torch.bfloat16:
+            raise ValueError("fp8 experts compute with bf16 activations: dtype must be torch.bfloat16")
         self.dtype = dtype
         self.device = torch.device("cuda", device)
         self.L, self.E, self.H, self.I, self.k = num_layers, num_experts, hidden, inter, top_k
@@ -84,7 +93,8 @@ class MoEEngine:
         self.max_tokens = max_tokens
         h = C.c_void_p()
         torch.cuda.set_device(self.device)
-        L.check(None, self.lib.b2m_ctx_create(C.byref(cfg), C.byref(h)))
+        fmt = L.WEIGHTS_FP8_E4M3_B128 if self.fp8 else L.WEIGHTS_MODEL_DTYPE
+        L.check(None, self.lib.b2m_ctx_create_ex(C.byref(cfg), fmt, C.byref(h)))
         self._h = h
         self._blobs: Dict[Tuple[int, int], torch.Tensor] = {}
         self._gates: Dict[int, torch.Tensor] = {}
@@ -94,6 +104,8 @@ class MoEEngine:
         else:
             nmat = 2 if expert_type == L.EXPERT_SWITCH else 3
             self.expert_bytes = nmat * hidden * inter * es
+        if self.fp8:
+            self.expert_bytes = F8.expert_blob_bytes(hidden, inter)
         self.shared_bytes = 3 * hidden * shared_inter * es
 
     # ------------------------------------------------------------------ lifecycle
@@ -126,10 +138,42 @@ class MoEEngine:
             raise ValueError(f"expert tensors total {off} bytes, expected {nbytes}")
         return blob
 
-    def register_expert(self, layer: int, expert: int, tensors: Sequence[torch.Tensor], pin: bool = True):
+    def _fp8_parts(self, tensors: Sequence[torch.Tensor], scales: Optional[Sequence[torch.Tensor]]) -> List[torch.Tensor]:
+        """The fp8 expert blob's parts as flat uint8 tensors: three e4m3 matrices, then their fp32 scale grids."""
+        if scales is None:
+            raise ValueError("an fp8 engine needs the three scale grids: scales=(s1, s2, s3)")
+        if len(tensors) != 3 or len(scales) != 3:
+            raise ValueError("an fp8 expert is three e4m3 matrices and three scale grids")
+        H, I = self.H, self.I
+        # nn.Linear [out, in]: Mixtral w1 | w2 | w3 = gate, down, up; DeepSeek gate | up | down
+        shapes = [(I, H), (H, I), (I, H)] if self.expert_type == L.EXPERT_MIXTRAL else [(I, H), (I, H), (H, I)]
+        parts = []
+        for t, shp in zip(tensors, shapes):
+            if t.dtype != torch.float8_e4m3fn or tuple(t.shape) != shp:
+                raise ValueError(f"expected a float8_e4m3fn {shp} matrix, got {t.dtype} {tuple(t.shape)}")
+            parts.append(t.detach().contiguous().view(torch.uint8).reshape(-1))
+        for s, shp in zip(scales, shapes):
+            want = (shp[0] // F8.BLOCK, shp[1] // F8.BLOCK)
+            if s.dtype != torch.float32 or tuple(s.shape) != want:
+                raise ValueError(f"expected a float32 {want} scale grid, got {s.dtype} {tuple(s.shape)}")
+            parts.append(s.detach().contiguous().view(torch.uint8).reshape(-1))
+        return parts
+
+    def register_expert(self, layer: int, expert: int, tensors: Sequence[torch.Tensor], pin: bool = True,
+                        scales: Optional[Sequence[torch.Tensor]] = None):
         """Host-backed expert (can be staged in and evicted).  tensors: Mixtral (w1,w2,w3),
-        DeepSeek (gate,up,down), Switch (wi,wo), NLLB/FSGPT (fc1,fc1_bias,fc2,fc2_bias) -- nn.Linear [out,in] layout."""
-        blob = self._pack(tensors, self.expert_bytes, pin)
+        DeepSeek (gate,up,down), Switch (wi,wo), NLLB/FSGPT (fc1,fc1_bias,fc2,fc2_bias) -- nn.Linear [out,in] layout.
+        fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids."""
+        if self.fp8:
+            blob = torch.zeros(self.expert_bytes, dtype=torch.uint8, pin_memory=pin)
+            off = 0
+            for part in self._fp8_parts(tensors, scales):
+                blob[off:off + part.numel()] = part.cpu()
+                off += part.numel()
+        elif scales is not None:
+            raise ValueError("scales are only taken by an fp8 engine (expert_dtype=torch.float8_e4m3fn)")
+        else:
+            blob = self._pack(tensors, self.expert_bytes, pin)
         self._blobs[(layer, expert)] = blob
         self._ck(self.lib.b2m_register_expert(self._h, layer, expert, C.c_void_p(blob.data_ptr()), blob.numel()))
 
@@ -151,16 +195,30 @@ class MoEEngine:
         self._ck(self.lib.b2m_expert_dev_ptr(self._h, layer, expert, C.byref(p)))
         if not p.value:
             return None
+        if self.fp8:   # the fp8 expert blob (fp8.py): e4m3 matrices, then fp32 scale grids
+            return _view(p.value, (self.expert_bytes,), torch.uint8, self.device)
         return _view(p.value, (self.expert_bytes // self.esize,), self.dtype, self.device)
 
-    def load_expert(self, layer: int, expert: int, tensors: Optional[Sequence[torch.Tensor]] = None):
+    def load_expert(self, layer: int, expert: int, tensors: Optional[Sequence[torch.Tensor]] = None,
+                    scales: Optional[Sequence[torch.Tensor]] = None):
         """HBM-only expert: claims a slot, pins it, fills it from `tensors` (any device) if given.
         Returns the flat device view of the slot so callers can initialise it in place.  Writes through the view must be
         issued (on the current stream) before the next forward of this layer; the second eager forward after the load packs
-        the slot for the decode GEMMs (pack_weights=True); to change the weights later, call load_expert again and write through the view it returns."""
+        the slot for the decode GEMMs (pack_weights=True); to change the weights later, call load_expert again and write through the view it returns.
+        fp8 engine: `tensors` are the three float8_e4m3fn matrices and `scales` their float32 grids; the view is uint8."""
+        if self.fp8 and tensors is not None:
+            parts = self._fp8_parts(tensors, scales)
+        elif scales is not None:
+            raise ValueError("scales go with the fp8 matrices of an fp8 engine")
         self._ck(self.lib.b2m_make_resident(self._h, layer, expert, 1 | 2, C.c_void_p(_stream_ptr())))
         v = self.expert_device_view(layer, expert)
-        if tensors is not None:
+        if self.fp8 and tensors is not None:
+            off = 0
+            for part in parts:
+                v[off:off + part.numel()].copy_(part)
+                off += part.numel()
+            v[off:].zero_()
+        elif tensors is not None:
             off = 0
             for t in tensors:
                 n = t.numel()
