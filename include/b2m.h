@@ -56,6 +56,24 @@ extern "C" {
 #define B2M_ROUTER_DEEPSEEK_GREEDY 1 /* models/modeling_deepseek/modeling_deepseek.py:467-483,508-512     */
 #define B2M_ROUTER_DEEPSEEK_GROUP 2  /* modeling_deepseek.py:484-505 (group_limited_greedy)               */
 #define B2M_ROUTER_SWITCH_TOP1 3     /* HF 4.x SwitchTransformersTop1Router (switch_transformers.py:76)   */
+/* DeepSeek-V3 MoEGate, topk_method "noaux_tc", scoring_func "sigmoid"
+ * (models/modeling_deepseek_v3/modeling_deepseek.py:466-527, built by models/deepseek.py:23-27).  Per token:
+ *   1. s = sigmoid(fp32 logits)                           (no softmax; 1 / (1 + exp(-x)) with an IEEE division)
+ *   2. choice[e] = s[e] + bias[e]                          bias = the layer's fp32 [E] e_score_correction_bias (b2m_set_gate_bias)
+ *   3. group score = top1 + top2 of the group's choices    (n_group groups of E / n_group experts); the topk_group best
+ *                                                          groups are kept
+ *   4. choices outside the kept groups become 0.0          (masked_fill(~mask, 0.0), not -inf: with negative biases a
+ *                                                          masked expert can win)
+ *   5. top_k experts by choice; their weights are the UNBIASED s
+ *   6. if top_k > 1 and norm_topk_prob: w /= (sum of the k weights, in selection order) + 1e-20; then ALWAYS
+ *      w *= routed_scaling_factor
+ * Ties at every stage (groups and experts) go to the lowest index.  Limits (b2m_ctx_create_ex, B2M_EINVAL otherwise):
+ * 1 <= n_group <= 32, E % n_group == 0, E / n_group >= 2, 1 <= topk_group <= n_group.
+ * router_in_kind: 0 = fused fp32 gate (B2M_WS_LOGITS holds fp32 logits), 1 = logits of any supported dtype (sigmoid
+ * applied here), 2 = fp32 sigmoid scores used as given.  B2M_WS_SCORES holds the unbiased sigmoid scores.  A routing call
+ * on a layer whose bias was never set returns B2M_ESTATE (whatever router_in_kind).  The combine is the DeepSeek one
+ * (models/deepseek.py:115-137). */
+#define B2M_ROUTER_DEEPSEEK_V3 4
 
 /* numerics of epilogue + combine */
 #define B2M_NUMERICS_REFERENCE 0 /* replay the reference's per-ATen-op rounding to the model dtype */
@@ -180,6 +198,11 @@ int b2m_register_expert(b2m_ctx* ctx, int layer, int expert, const void* host_bl
 int b2m_register_shared(b2m_ctx* ctx, int layer, const void* host_blob, size_t bytes); /* deepseek.py:39-45 */
 /* router weight [E,H] on the device, dtype cfg.gate_dtype (mixtral.py:30 `self.gate`; MoEGate.weight) */
 int b2m_set_gate(b2m_ctx* ctx, int layer, const void* dev_gate_weight);
+/* B2M_ROUTER_DEEPSEEK_V3 only: the layer's e_score_correction_bias, fp32 [E] on the device (MoEGate.e_score_correction_bias,
+ * modeling_deepseek.py:455-458).  Borrowed like the gate weight: it must stay valid, and is read by every routing call of
+ * the layer (and by the look-ahead prediction made from the layer before it).  B2M_EINVAL for a layer out of range, a null
+ * pointer, or a context whose router is not B2M_ROUTER_DEEPSEEK_V3. */
+int b2m_set_gate_bias(b2m_ctx* ctx, int layer, const float* dev_bias);
 
 /* replaces: HostMemoryPool / cudaHostAlloc per node (core/memory/memory_pool.cpp:29-83) */
 int b2m_host_pin(b2m_ctx* ctx, void* host_ptr, size_t bytes);
@@ -233,7 +256,7 @@ int b2m_check_errors(b2m_ctx* ctx, void* stream);
 #define B2M_WS_XP 6         /* dtype [T*k,H] */
 #define B2M_WS_HMID 7       /* dtype [T*k,I] */
 #define B2M_WS_Y 8          /* fp32  [T*k,H] */
-#define B2M_WS_SCORES 9     /* fp32  [T,E] softmax probabilities */
+#define B2M_WS_SCORES 9     /* fp32  [T,E] softmax probabilities (B2M_ROUTER_DEEPSEEK_V3: unbiased sigmoid scores) */
 #define B2M_WS_LOGITS 10    /* router logits computed by the fused gate: model dtype (Mixtral) or fp32 */
 int b2m_ws_ptr(b2m_ctx* ctx, int which, void** dev_ptr);
 

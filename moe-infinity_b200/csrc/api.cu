@@ -138,6 +138,7 @@ struct b2m_ctx {
   int* h_stage = nullptr;  // pinned [STAGE_RING][E]
   int stage_pos = 0;
   std::vector<const void*> gate_w;  // per layer device pointers
+  std::vector<const float*> gate_bias;  // B2M_ROUTER_DEEPSEEK_V3: per layer e_score_correction_bias [E] (device, borrowed)
 
   // workspace
   int cap_T = 0, cap_R = 0;
@@ -689,6 +690,7 @@ RouteParams base_route_params(b2m_ctx* c, int layer, const void* x, int T, int s
   p.router = f.router;
   p.n_group = f.n_group; p.topk_group = f.topk_group; p.norm_topk_prob = f.norm_topk_prob;
   p.routed_scaling_factor = f.routed_scaling_factor;
+  p.gate_bias = c->gate_bias[layer];
   p.seq_len = seq_len > 0 ? seq_len : T;
   p.expert_capacity = f.expert_capacity;
   p.scores = c->d_scores;
@@ -762,7 +764,17 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
     make_fp8_shape(&shape);
   }
-  if (cfg->router < 0 || cfg->router > 3) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router < 0 || cfg->router > 4) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router == B2M_ROUTER_DEEPSEEK_V3) {
+    if (cfg->n_group < 1 || cfg->n_group > 32 || cfg->num_experts % cfg->n_group)
+      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: n_group=%d must be in 1..32 and divide num_experts=%d", cfg->n_group,
+                  cfg->num_experts);
+    if (cfg->num_experts / cfg->n_group < 2)
+      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: a group needs at least 2 experts (top-2 group score), got %d",
+                  cfg->num_experts / cfg->n_group);
+    if (cfg->topk_group < 1 || cfg->topk_group > cfg->n_group)
+      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: topk_group=%d must be in 1..n_group=%d", cfg->topk_group, cfg->n_group);
+  }
   if (cfg->cache_policy < B2M_CACHE_REFERENCE || cfg->cache_policy > B2M_CACHE_ACTIVATION_AWARE) return fail(nullptr, B2M_EINVAL, "bad cache_policy");
   if (cfg->freq_alpha < 0.f || cfg->freq_alpha > 1.f) return fail(nullptr, B2M_EINVAL, "freq_alpha must be in [0,1]");
   if (cfg->router == B2M_ROUTER_SWITCH_TOP1 && cfg->top_k != 1) return fail(nullptr, B2M_EINVAL, "switch router needs top_k=1");
@@ -848,6 +860,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   c->h_slot_of.assign((size_t)L * E, -1);
   c->row_dirty.assign(L, 1);
   c->gate_w.assign(L, nullptr);
+  c->gate_bias.assign(L, nullptr);
   CKC(cudaMalloc((void**)&c->d_slot_of, sizeof(int) * L * E));
   CKC(cudaMemset(c->d_slot_of, 0xff, sizeof(int) * L * E));
   CKC(cudaHostAlloc((void**)&c->h_stage, sizeof(int) * STAGE_RING * E, cudaHostAllocDefault));
@@ -1007,6 +1020,17 @@ int b2m_set_gate(b2m_ctx* c, int layer, const void* dev_gate_weight) {
   return B2M_OK;
 }
 
+int b2m_set_gate_bias(b2m_ctx* c, int layer, const float* dev_bias) {
+  int r = check_layer(c, layer);
+  if (r) return r;
+  if (c->cfg.router != B2M_ROUTER_DEEPSEEK_V3)
+    return fail(c, B2M_EINVAL, "b2m_set_gate_bias: only a deepseek_v3 router (%d) has a correction bias, this context's router is %d",
+                B2M_ROUTER_DEEPSEEK_V3, c->cfg.router);
+  if (!dev_bias) return fail(c, B2M_EINVAL, "b2m_set_gate_bias: dev_bias is null");
+  c->gate_bias[layer] = dev_bias;
+  return B2M_OK;
+}
+
 int b2m_host_pin(b2m_ctx* c, void* host_ptr, size_t bytes) {
   if (!c || !host_ptr) return B2M_EINVAL;
   CK(c, cudaHostRegister(host_ptr, bytes, cudaHostRegisterDefault));
@@ -1117,6 +1141,8 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
   }
   if (c->cfg.router == B2M_ROUTER_SWITCH_TOP1 && (p.seq_len <= 0 || T % p.seq_len))
     return fail(c, B2M_EINVAL, "T=%d is not a multiple of seq_len=%d", T, p.seq_len);
+  if (c->cfg.router == B2M_ROUTER_DEEPSEEK_V3 && !p.gate_bias)
+    return fail(c, B2M_ESTATE, "layer %d has no correction bias (b2m_set_gate_bias)", layer);
   plan_gemm(c, T);
   if (c->cur_ksplit > 1) { p.y_zero = c->d_y; p.y_zero_elems = (size_t)T * c->cfg.top_k * c->cfg.hidden; }
   // small batches, all experts resident: let the last gate/top-k CTA publish the offsets so that the gate/up GEMM can be
@@ -1144,13 +1170,15 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
   c->ep_fused_last = p.ep_fused != 0;
   c->last_counts_valid = false;
   // router-logit driven prefetch: the next layer's router applied to THIS layer's input predicts which experts the next
-  // layer will want; the counts ride back with this layer's own counts (b2m_run_experts reads both in one synchronisation)
+  // layer will want; the counts ride back with this layer's own counts (b2m_run_experts reads both in one synchronisation).
+  // DeepSeek-V3 predicts with the next layer's bias too (top-k of raw logits is not its choice); no bias, no prediction.
   c->look_pending = false;
   const int nxt = (layer + 1) % c->cfg.num_layers;
   if (c->cfg.lookahead_prefetch && c->offload && !c->ep_mode && T >= 1 && T <= 256 && c->cfg.dtype != B2M_DTYPE_F32 &&
-      c->cfg.num_layers > 1 && c->gate_w[nxt]) {
+      c->cfg.num_layers > 1 && c->gate_w[nxt] && (c->cfg.router != B2M_ROUTER_DEEPSEEK_V3 || c->gate_bias[nxt])) {
     RouteParams q = p;
     q.gate_w = c->gate_w[nxt];
+    q.gate_bias = c->gate_bias[nxt];
     q.logits = nullptr;
     CK(c, cudaMemsetAsync(c->d_look, 0, sizeof(int) * c->cfg.num_experts, st));
     CK(c, launch_lookahead_counts(q, c->d_look, st));

@@ -16,6 +16,7 @@ enum : int {
   ROUTER_DEEPSEEK_GREEDY = 1,  // modeling_deepseek.py:467-483,508-512
   ROUTER_DEEPSEEK_GROUP = 2,   // modeling_deepseek.py:484-505
   ROUTER_SWITCH_TOP1 = 3,      // HF 4.x SwitchTransformersTop1Router (switch_transformers.py:76)
+  ROUTER_DEEPSEEK_V3 = 4,      // modeling_deepseek_v3/modeling_deepseek.py:466-527 (sigmoid, noaux_tc)
 };
 // combine kinds (which reference combine loop is restated)
 enum : int {
@@ -175,6 +176,7 @@ struct RouteParams {
   int router;                // ROUTER_*
   int n_group, topk_group, norm_topk_prob;
   float routed_scaling_factor;
+  const float* gate_bias;    // ROUTER_DEEPSEEK_V3: the layer's e_score_correction_bias [E] fp32 (required)
   int seq_len, expert_capacity;   // Switch only
   // outputs (workspace)
   float* scores;             // [T,E] fp32 softmax probabilities (optional, may be null)
@@ -203,8 +205,8 @@ struct RouteParams {
   unsigned long long* tl;    // optional timeline slots: [0] gate/top-k start, [1] its end, [2] permute start, [3] permute end
 };
 cudaError_t launch_route(const RouteParams& p, cudaStream_t st);
-// look-ahead: top-k of the NEXT layer's router (p.gate_w = its weight) on this layer's input p.x -> counts_out[E] += 1 per
-// selected (token, expert); counts_out must be zero.  T <= 256.
+// look-ahead: top-k of the NEXT layer's router (p.gate_w = its weight; DeepSeek-V3: p.gate_bias = its bias) on this layer's
+// input p.x -> counts_out[E] += 1 per selected (token, expert); counts_out must be zero.  T <= 256.
 cudaError_t launch_lookahead_counts(const RouteParams& p, int* counts_out, cudaStream_t st);
 // routing from a caller-supplied dense mask (reference compat: ExpertDispatcher::SetInputs + per-expert gather,
 // core/parallel/expert_dispatcher.h:66-70, expert_dispatcher.cpp:274-285)

@@ -3,6 +3,7 @@
 // Replaces, with zero host synchronisation:
 //   * moe_infinity/models/mixtral.py:46-65        gate GEMM, softmax, topk, renorm, dense [T,E] mask build
 //   * modeling_deepseek.py:463-512 + deepseek.py:76-91   MoEGate and its mask build
+//   * modeling_deepseek_v3/modeling_deepseek.py:466-527  DeepSeek-V3 MoEGate (sigmoid, correction bias, noaux_tc)
 //   * distributed/expert_executor.py:34-44         per-expert token counts (.cpu() sync in the reference)
 //   * core/parallel/expert_dispatcher.cpp:274-285  per-expert boolean-mask gather (nonzero + index_select)
 //   * mixtral.py:96-101 / deepseek.py:123-136 / switch_transformers.py:99-109   per-expert masked combine
@@ -283,10 +284,114 @@ __global__ void __launch_bounds__(256, 2) gate_logits_kernel(const RouteParams p
 }
 
 // --------------------------------------------------------------------------------------
+// DeepSeek-V3 noaux_tc selection (modeling_deepseek_v3/modeling_deepseek.py:483-513) for one token, one warp, lane owns
+// experts lane + 32*i.  s = unbiased sigmoid scores, bias = the layer's e_score_correction_bias [E].
+//   choice = s + bias; group score = top1 + top2 of the group's choices; the topk_group best groups are kept; choices
+//   outside them become 0.0 (masked_fill, not -inf); k rounds of arg-max over the choices.  Ties -> lowest index.
+// Leaves winner j (selection order) in s_scr[MAX_K + j] (int bits) and its UNBIASED score in s_scr[j].
+// Used by the routing kernels and by the look-ahead predictor.
+// --------------------------------------------------------------------------------------
+__device__ __forceinline__ void v3_select_warp(const RouteParams& p, const float (&s)[MAX_PL], const float* __restrict__ bias,
+                                               float* s_scr /*[E] smem scratch*/) {
+  const int lane = threadIdx.x & 31;
+  const int E = p.E;
+  const int gsz = E / p.n_group;
+  float c[MAX_PL];
+#pragma unroll
+  for (int i = 0; i < MAX_PL; ++i) {
+    const int e = lane + 32 * i;
+    c[i] = e < E ? __fadd_rn(s[i], bias[e]) : -INFINITY;
+    if (e < E) s_scr[e] = c[i];
+  }
+  __syncwarp();
+  // group score: sum of the two largest choices of the group (topk(2).sum(); duplicates count twice)
+  float gsc = -INFINITY;
+  if (lane < p.n_group) {
+    float t1 = -INFINITY, t2 = -INFINITY;
+    for (int j = 0; j < gsz; ++j) {
+      const float cv = s_scr[lane * gsz + j];
+      if (cv > t1) { t2 = t1; t1 = cv; } else if (cv > t2) { t2 = cv; }
+    }
+    gsc = __fadd_rn(t1, t2);
+  }
+  uint32_t allowed = 0;
+  for (int r = 0; r < p.topk_group; ++r) {
+    float bv = lane < p.n_group ? gsc : -INFINITY;
+    int bi = lane < p.n_group ? lane : 0x7fffffff;
+    warp_argmax(bv, bi);
+    allowed |= 1u << bi;
+    if (lane == bi) gsc = -INFINITY;
+  }
+#pragma unroll
+  for (int i = 0; i < MAX_PL; ++i) {
+    const int e = lane + 32 * i;
+    if (e < E && !((allowed >> (e / gsz)) & 1u)) c[i] = 0.0f;   // masked_fill(~score_mask, 0.0)
+  }
+  __syncwarp();   // s_scr is reused for the winners below
+  uint32_t taken = 0;
+#pragma unroll 1
+  for (int j = 0; j < p.k; ++j) {
+    float bv = -INFINITY, sw = 0.f;   // sw: the candidate's unbiased score travels with it (gather(scores, topk_idx))
+    int bi = 0x7fffffff;
+#pragma unroll
+    for (int i = 0; i < MAX_PL; ++i) {
+      const int e = lane + 32 * i;
+      if (e < E && !((taken >> i) & 1u) && (c[i] > bv || bi == 0x7fffffff)) { bv = c[i]; bi = e; sw = s[i]; }
+    }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {   // warp_argmax carrying sw
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, d);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, d);
+      const float os = __shfl_xor_sync(0xffffffffu, sw, d);
+      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; sw = os; }
+    }
+    if ((bi & 31) == lane) taken |= 1u << (bi >> 5);
+    if (lane == 0) {
+      s_scr[j] = sw;
+      s_scr[MAX_K + j] = __int_as_float(bi);
+    }
+  }
+  __syncwarp();
+}
+
+// sigmoid exactly as PyTorch's CUDA kernel computes it in fp32: 1 / (1 + exp(-x)), IEEE division
+__device__ __forceinline__ float sigmoid_ref(float x) { return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x))); }
+
+// DeepSeek-V3 gate for one token: sigmoid (unless scores come in), selection, weights (modeling_deepseek.py:475-526)
+// (inlined: a call would copy the kernel's RouteParams to a 1.2 KB stack frame to pass it by reference)
+__device__ __forceinline__ void route_token_v3(const RouteParams& p, int t, const float* s_in, bool in_are_scores,
+                                               float* s_scr, int* out_idx, float* out_w) {
+  const int lane = threadIdx.x & 31;
+  const int E = p.E;
+  float s[MAX_PL];
+#pragma unroll
+  for (int i = 0; i < MAX_PL; ++i) {
+    const int e = lane + 32 * i;
+    s[i] = e < E ? (in_are_scores ? s_in[e] : sigmoid_ref(s_in[e])) : 0.f;
+    if (p.scores && e < E) p.scores[(size_t)t * E + e] = s[i];
+  }
+  v3_select_warp(p, s, p.gate_bias, s_scr);
+  // weights: unbiased scores, normalised by their sum in selection order (k > 1 and norm_topk_prob), then ALWAYS scaled
+  float denom = 0.f;
+  for (int j = 0; j < p.k; ++j) denom = __fadd_rn(denom, s_scr[j]);
+  if (lane < p.k) {
+    float w = s_scr[lane];
+    if (p.k > 1 && p.norm_topk_prob) w = __fdiv_rn(w, __fadd_rn(denom, 1e-20f));
+    out_idx[lane] = __float_as_int(s_scr[MAX_K + lane]);
+    out_w[lane] = __fmul_rn(w, p.routed_scaling_factor);
+  }
+  __syncwarp();
+}
+
+// --------------------------------------------------------------------------------------
 // K1: softmax + top-k (+renorm) for one token (one warp, lane owns experts lane, lane+32, ...)
 // --------------------------------------------------------------------------------------
 __device__ void route_token_warp(const RouteParams& p, int t, const float* s_in /*[E] logits or scores (smem)*/,
                                  bool in_are_scores, float* s_scr /*[E] smem scratch*/, int* out_idx, float* out_w) {
+  if (p.router == ROUTER_DEEPSEEK_V3) {
+    route_token_v3(p, t, s_in, in_are_scores, s_scr, out_idx, out_w);
+    return;
+  }
   const int lane = threadIdx.x & 31;
   const int E = p.E;
   float v[MAX_PL];
@@ -958,8 +1063,11 @@ static bool route_args_ok(const RouteParams& p);
 // Look-ahead routing (cfg.lookahead_prefetch): one CTA per token applies the NEXT layer's router weight (p.gate_w) to this
 // layer's input row and counts its top-k choice per expert.  softmax is monotonic, so top-k of the logits is the top-k of
 // the scores (ties -> lowest index, like every routing kernel here); weights are not needed for a prefetch hint.
+// DeepSeek-V3: the bias and the group rule change the order, so the next layer's full V3 selection runs (p.gate_bias =
+// that layer's bias).
 __global__ void __launch_bounds__(RT_THREADS) lookahead_counts_kernel(const RouteParams p, int* __restrict__ counts_out) {
   __shared__ float s_logits[MAX_PL * 32];
+  __shared__ float s_scr[MAX_PL * 32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t = blockIdx.x;
   for (int e = warp; e < p.E; e += RT_WARPS) {
@@ -967,7 +1075,16 @@ __global__ void __launch_bounds__(RT_THREADS) lookahead_counts_kernel(const Rout
     if (lane == 0) s_logits[e] = v;
   }
   __syncthreads();
-  if (warp == 0) {
+  if (warp == 0 && p.router == ROUTER_DEEPSEEK_V3) {
+    float s[MAX_PL];
+#pragma unroll
+    for (int i = 0; i < MAX_PL; ++i) {
+      const int e = lane + 32 * i;
+      s[i] = e < p.E ? sigmoid_ref(s_logits[e]) : 0.f;
+    }
+    v3_select_warp(p, s, p.gate_bias, s_scr);
+    if (lane < p.k) atomicAdd(counts_out + __float_as_int(s_scr[MAX_K + lane]), 1);
+  } else if (warp == 0) {
     for (int j = 0; j < p.k; ++j) {
       float best = -INFINITY;
       int bi = 0x7fffffff;
@@ -984,7 +1101,8 @@ __global__ void __launch_bounds__(RT_THREADS) lookahead_counts_kernel(const Rout
 }
 
 cudaError_t launch_lookahead_counts(const RouteParams& p, int* counts_out, cudaStream_t st) {
-  if (!route_args_ok(p) || !p.gate_w || !p.x || !counts_out || p.T < 1 || p.T > FUSED_MAX_T || p.dtype == DT_F32)
+  if (!route_args_ok(p) || !p.gate_w || !p.x || !counts_out || p.T < 1 || p.T > FUSED_MAX_T || p.dtype == DT_F32 ||
+      (p.router == ROUTER_DEEPSEEK_V3 && !p.gate_bias))
     return cudaErrorInvalidValue;
   lookahead_counts_kernel<<<p.T, RT_THREADS, 0, st>>>(p, counts_out);
   return cudaGetLastError();
@@ -999,11 +1117,14 @@ static bool route_args_ok(const RouteParams& p) {
   return p.E >= 1 && p.E <= MAX_PL * 32 && p.k >= 1 && p.k <= MAX_K && p.k <= p.E && p.H % 8 == 0 && p.T >= 0 &&
          (p.router != ROUTER_DEEPSEEK_GROUP || (p.n_group >= 1 && p.n_group <= 32 && p.E % p.n_group == 0 &&
                                                  p.topk_group >= 1 && p.topk_group <= p.n_group)) &&
+         (p.router != ROUTER_DEEPSEEK_V3 || (p.n_group >= 1 && p.n_group <= 32 && p.E % p.n_group == 0 &&
+                                              p.E / p.n_group >= 2 && p.topk_group >= 1 && p.topk_group <= p.n_group)) &&
          (p.router != ROUTER_SWITCH_TOP1 || (p.k == 1 && p.seq_len > 0 && p.T % p.seq_len == 0));
 }
 
 cudaError_t launch_route(const RouteParams& p, cudaStream_t st) {
   if (!route_args_ok(p)) return cudaErrorInvalidValue;
+  if (p.router == ROUTER_DEEPSEEK_V3 && !p.gate_bias) return cudaErrorInvalidValue;   // the V3 gate always has a bias
   if (p.dtype == DT_F32 && (!p.logits || p.ep_dispatch)) return cudaErrorInvalidValue;   // fp32 models: router logits/scores come in
   if (p.T == 0) return cudaMemsetAsync(p.offsets, 0, sizeof(int) * (p.E + 1), st);
   if (p.T <= FUSED_MAX_T) {

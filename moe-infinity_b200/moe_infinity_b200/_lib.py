@@ -14,7 +14,7 @@ B2M_OK, B2M_EINVAL, B2M_ECUDA, B2M_ENOMEM, B2M_ESTATE, B2M_EUNSUPPORTED, B2M_EIO
 STORE_NO_ODIRECT = 1
 DTYPE_BF16, DTYPE_F32, DTYPE_F16, DTYPE_FP8 = 0, 1, 2, 3
 EXPERT_SWITCH, EXPERT_SWITCH_GATED, EXPERT_NLLB, EXPERT_FSGPT, EXPERT_MIXTRAL, EXPERT_DEEPSEEK = 0, 1, 2, 3, 4, 5
-ROUTER_MIXTRAL, ROUTER_DEEPSEEK_GREEDY, ROUTER_DEEPSEEK_GROUP, ROUTER_SWITCH_TOP1 = 0, 1, 2, 3
+ROUTER_MIXTRAL, ROUTER_DEEPSEEK_GREEDY, ROUTER_DEEPSEEK_GROUP, ROUTER_SWITCH_TOP1, ROUTER_DEEPSEEK_V3 = 0, 1, 2, 3, 4
 NUMERICS_REFERENCE, NUMERICS_FP32 = 0, 1
 CACHE_REFERENCE, CACHE_SLOTS, CACHE_ACTIVATION_AWARE = 0, 1, 2
 WEIGHTS_MODEL_DTYPE, WEIGHTS_FP8_E4M3_B128 = 0, 1
@@ -54,6 +54,7 @@ SYMBOLS = [
     ("b2m_register_expert", _I, [_VP, _I, _I, _VP, _SZ]),
     ("b2m_register_shared", _I, [_VP, _I, _VP, _SZ]),
     ("b2m_set_gate", _I, [_VP, _I, _VP]),
+    ("b2m_set_gate_bias", _I, [_VP, _I, _VP]),
     ("b2m_host_pin", _I, [_VP, _VP, _SZ]),
     ("b2m_host_unpin", _I, [_VP, _VP]),
     ("b2m_make_resident", _I, [_VP, _I, _I, _I, _VP]),

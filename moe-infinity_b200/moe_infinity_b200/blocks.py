@@ -79,27 +79,52 @@ class SyncMixtralSparseMoeBlock(nn.Module):
             self.expert_prefetcher.prefetch_experts(self.layer_id, m)
 
 
+def _engine_of(executor):
+    d = executor.expert_dispatcher
+    return d.engine if hasattr(d, "engine") else d
+
+
 class DeepseekMoEBlock(nn.Module):
-    """moe_infinity/models/deepseek.py:8-137 (DeepSeek-V2 gate: modeling_deepseek.py:436-512)."""
+    """moe_infinity/models/deepseek.py:8-137 (DeepSeek-V2 gate: modeling_deepseek.py:436-512; DeepSeek-V3 gate when
+    config.model_type == "deepseek_v3" or config.topk_method == "noaux_tc": modeling_deepseek_v3/modeling_deepseek.py:436-527,
+    routed by an engine built with ROUTER_DEEPSEEK_V3)."""
     layer_id: int = None
 
     def __init__(self, config):
         super().__init__()
         self.config = config
         self.num_experts_per_tok = config.num_experts_per_tok
+        self.v3 = getattr(config, "model_type", None) == "deepseek_v3" or getattr(config, "topk_method", None) == "noaux_tc"
         self.gate_weight = nn.Parameter(torch.empty((config.n_routed_experts, config.hidden_size)))
         nn.init.kaiming_uniform_(self.gate_weight, a=5 ** 0.5)
+        if self.v3:   # MoEGate.e_score_correction_bias (modeling_deepseek_v3/modeling_deepseek.py:455-458)
+            self.e_score_correction_bias = nn.Parameter(torch.zeros(config.n_routed_experts, dtype=torch.float32))
+        self._bias_handed = None
         self.expert_executor = None
         self.expert_prefetcher = None
         self.expert_predictor = None
+
+    def _hand_bias(self):
+        """Give the engine this layer's correction bias, once per (engine, tensor, version): a captured graph keeps reading
+        the tensor the engine holds."""
+        eng = _engine_of(self.expert_executor)
+        b = self.e_score_correction_bias
+        key = (id(eng), b.data_ptr(), b._version)
+        if self._bias_handed != key:
+            eng.set_gate_bias(self.layer_id, b)
+            self._bias_handed = key
 
     def forward(self, hidden_states):
         orig_shape = hidden_states.shape
         x = hidden_states.view(-1, orig_shape[-1])
         logits = F.linear(x.type(torch.float32), self.gate_weight.type(torch.float32), None)   # modeling_deepseek.py:467-471
-        scores = logits.softmax(dim=-1, dtype=torch.float32)                                   # :473
         if not _is_fast(self.expert_executor):
             raise RuntimeError("DeepseekMoEBlock needs the CUDA executor (expert_executor.moe_forward)")
+        if self.v3:
+            scores = logits.sigmoid()                                  # modeling_deepseek_v3/modeling_deepseek.py:475-476
+            self._hand_bias()                                          # bias, groups, top-k, weights: in the engine
+        else:
+            scores = logits.softmax(dim=-1, dtype=torch.float32)                               # :473
         out = self.expert_executor.moe_forward(self.layer_id, x, scores=scores)   # top-k, experts, combine, shared experts
         return out.view(orig_shape)
 

@@ -98,6 +98,7 @@ class MoEEngine:
         self._h = h
         self._blobs: Dict[Tuple[int, int], torch.Tensor] = {}
         self._gates: Dict[int, torch.Tensor] = {}
+        self._biases: Dict[int, torch.Tensor] = {}
         es = self.esize = 4 if dtype == torch.float32 else 2   # fp32 experts (dtype int 1) run on the CUDA-core fp32 path
         if expert_type in (L.EXPERT_NLLB, L.EXPERT_FSGPT):     # fc1 | fc1_bias | fc2 | fc2_bias (expert_module.cpp:70-77)
             self.expert_bytes = 2 * hidden * inter * es + (inter + hidden) * es
@@ -236,6 +237,17 @@ class MoEEngine:
         w = weight.detach().to(self.device, self.gate_dtype).contiguous()
         self._gates[layer] = w
         self._ck(self.lib.b2m_set_gate(self._h, layer, C.c_void_p(w.data_ptr())))
+
+    def set_gate_bias(self, layer: int, bias: torch.Tensor):
+        """DeepSeek-V3 router (ROUTER_DEEPSEEK_V3): the layer's e_score_correction_bias [E].  fp32, or bf16 (upcast exactly;
+        a block cast with .to(bf16) holds it in bf16)."""
+        if self.router != L.ROUTER_DEEPSEEK_V3:
+            raise ValueError("set_gate_bias needs a DeepSeek-V3 engine (router=ROUTER_DEEPSEEK_V3)")
+        if bias.dtype not in (torch.float32, torch.bfloat16) or tuple(bias.shape) != (self.E,):
+            raise ValueError(f"expected a float32 or bfloat16 [{self.E}] bias, got {bias.dtype} {tuple(bias.shape)}")
+        b = bias.detach().to(self.device, torch.float32).contiguous()
+        self._biases[layer] = b                # borrowed by the context: keep it alive
+        self._ck(self.lib.b2m_set_gate_bias(self._h, layer, C.c_void_p(b.data_ptr())))
 
     # ------------------------------------------------------------------ hot path
     def _router_args(self, router_logits, scores):
