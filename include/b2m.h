@@ -185,6 +185,25 @@ int b2m_ctx_destroy(b2m_ctx* ctx);
                                        Mixtral (4) and DeepSeek (5); hidden and inter multiples of 128; gemm_impl 0 or 2 (the
                                        12-bit packed copy of gemm_impl 0 is never made).  The expert-parallel entry points
                                        return B2M_EUNSUPPORTED on such a context. */
+/* (2 and 3 are not weight formats: B2M_EINVAL) */
+#define B2M_WEIGHTS_INT4_G128 4     /* 4-bit integer matrices with a bf16 scale and a 4-bit zero point per 128 inputs (W4A16,
+                                       asymmetric group quantisation).  Each routed matrix (nn.Linear [out,in], row-major) is
+                                       codes q[r][c] in 0..15, scales s[r][c/128] (bf16) and zero points z[r][c/128] in 0..15.
+                                       The experts compute exactly what the bf16 engine computes on
+                                         W[r][c] = bf16(s[r][c/128] * (q[r][c] - z[r][c/128]))
+                                       -- the product is exact in fp32 and is rounded once to nearest-even, subnormals kept
+                                       (torch: `(s_expanded.float() * (q.float() - z_expanded.float())).to(torch.bfloat16)`);
+                                       the GEMMs dequantise inside the kernel, so results are bit-identical to a bf16 context
+                                       holding those W.
+                                       Expert blob (b2m_register_expert, b2m_expert_dev_ptr), 3*H*I/2 + 3*(H*I/128)*4 bytes,
+                                       no padding: (1) the three code matrices in the model's tensor order (Mixtral w1|w2|w3,
+                                       DeepSeek gate|up|down), each [rows][cols/2] bytes, byte c/2 holding column c in its low
+                                       nibble (c even) or its high nibble (c odd); (2) their three group grids in the same
+                                       order, one uint32 per (row r, group g = c/128): bits 0..15 the bf16 bits of s, bits
+                                       16..19 z, the other bits ignored; the grid is tile-major, the word of (r, g) at index
+                                       ((r/128) * (cols/128) + g) * 128 + r%128.  Activations, outputs, workspaces and the
+                                       router stay bf16; DeepSeek shared experts stay bf16.  Restrictions (B2M_EUNSUPPORTED
+                                       with a message) and the expert-parallel refusal: as B2M_WEIGHTS_FP8_E4M3_B128. */
 /* b2m_ctx_create with the routed experts stored in `weight_format` (B2M_WEIGHTS_*; any other value: B2M_EINVAL) */
 int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out);
 

@@ -29,6 +29,7 @@
 #include "../../include/b2m.h"
 #include "b2m_internal.h"
 #include "fp8_weights.cuh"
+#include "int4_weights.cuh"
 
 using namespace b2m;
 
@@ -78,7 +79,8 @@ struct ExpertShape {
   bool has_bias = false;          // fc1 | fc1_bias | fc2 | fc2_bias (NLLB / FSGPT)
   size_t off_bias1 = 0, off_bias2 = 0;
   bool fp8 = false;               // e4m3 matrices + fp32 128x128 block-scale grids (fp8_weights.cuh)
-  size_t sc_gate = 0, sc_up = 0, sc_down = 0;   // fp8: byte offsets of the three scale grids
+  bool int4 = false;              // 4-bit code matrices + tile-major group grids (int4_weights.cuh)
+  size_t sc_gate = 0, sc_up = 0, sc_down = 0;   // fp8 / int4: byte offsets of the three scale / group grids
 };
 
 struct Arena {
@@ -183,6 +185,7 @@ struct b2m_ctx {
 
   int cur_ksplit = 1, cur_nt = 16, cur_nt_dn = 16, cur_T = 0;   // token-tile widths of the up (K3) and down (K4) GEMMs
   bool fp8 = false;           // routed experts in B2M_WEIGHTS_FP8_E4M3_B128 (arena.shape.fp8)
+  bool int4 = false;          // routed experts in B2M_WEIGHTS_INT4_G128 (arena.shape.int4)
   bool ep_mode = false;       // experts of other ranks are simply absent (never an error)
   // 12-bit packed copy of the routed arena (weight_pack.cuh; same slot index), read by the decode GEMMs.  Allocated by the first
   // eager forward that packs, if the device keeps PK_RESERVE free beside it.  d_ok[slot]: bit b = matrix b (gate, up, down)
@@ -306,6 +309,23 @@ void make_fp8_shape(ExpertShape* s) {
   s->bytes = f8::expert_blob_bytes(s->H, s->I);
 }
 
+// routed experts of an int4 context: the model's matrices as 4-bit codes, then their group grids (int4_weights.cuh).  make_shape
+// ran with one-byte elements, so off_* / (H * I) is each matrix's place in the blob.
+void make_int4_shape(ExpertShape* s) {
+  const size_t m = (size_t)s->H * (size_t)s->I;
+  const int ig = (int)(s->off_gate / m), iu = (int)(s->off_up / m), id = (int)(s->off_down / m);
+  s->int4 = true;
+  s->off_gate = i4::code_offset(s->H, s->I, ig);
+  s->off_up = i4::code_offset(s->H, s->I, iu);
+  s->off_down = i4::code_offset(s->H, s->I, id);
+  s->sc_gate = i4::grid_offset(s->H, s->I, ig);
+  s->sc_up = i4::grid_offset(s->H, s->I, iu);
+  s->sc_down = i4::grid_offset(s->H, s->I, id);
+  s->bytes = i4::expert_blob_bytes(s->H, s->I);
+}
+
+// tensor-map element kind of the int4 code matrices (uint8 elements, 32-byte rows, SWIZZLE_32B: int4_weights.cuh)
+constexpr int MAP_INT4_CODES = -4;
 // dtype B2M_DTYPE_FP8_E4M3: e4m3 matrices as uint8 elements, 64-byte rows (SWIZZLE_64B, fp8_weights.cuh)
 int encode_map(b2m_ctx* c, CUtensorMap* tm, int dtype, void* base, int rank, const uint64_t* dims,
                const uint64_t* strides_bytes /*rank-1*/, const uint32_t* box) {
@@ -314,11 +334,12 @@ int encode_map(b2m_ctx* c, CUtensorMap* tm, int dtype, void* base, int rank, con
   cuuint32_t b[3], es[3];
   for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; b[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  const bool u8 = dtype == B2M_DTYPE_FP8_E4M3;
+  const bool u4 = dtype == MAP_INT4_CODES, u8 = dtype == B2M_DTYPE_FP8_E4M3 || u4;
   CUtensorMapDataType dt = u8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                          : dtype == B2M_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapSwizzle swz = u4 ? CU_TENSOR_MAP_SWIZZLE_32B : u8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = c->encode(tm, dt, (cuuint32_t)rank, base, gdim, gstr, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         u8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(c, B2M_ECUDA, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
   return B2M_OK;
@@ -332,20 +353,23 @@ int build_arena_maps(b2m_ctx* c, Arena* a) {
 }
 int build_arena_maps_box(b2m_ctx* c, Arena* a, uint32_t box_rows, CUtensorMap* tg, CUtensorMap* tu, CUtensorMap* td) {
   const ExpertShape& s = a->shape;
-  const uint32_t box[3] = {64, box_rows, 1};   // 64 k: the GEMM's k-block for every element size
-  const int dt = s.fp8 ? B2M_DTYPE_FP8_E4M3 : c->cfg.dtype;
-  const uint64_t es = s.fp8 ? 1 : 2;
+  // 64 k: the GEMM's k-block for every element size (int4: 32 bytes of two codes each)
+  const uint32_t box[3] = {s.int4 ? (uint32_t)i4::ROW_BYTES : 64u, box_rows, 1};
+  const int dt = s.int4 ? MAP_INT4_CODES : s.fp8 ? B2M_DTYPE_FP8_E4M3 : c->cfg.dtype;
+  const uint64_t es = s.fp8 ? 1 : 2;   // bytes per element (int4: per two codes, counted below in bytes)
+  const uint64_t kH = s.int4 ? (uint64_t)s.H / 2 : (uint64_t)s.H, kI = s.int4 ? (uint64_t)s.I / 2 : (uint64_t)s.I;
+  const uint64_t rH = s.int4 ? kH : (uint64_t)s.H * es, rI = s.int4 ? kI : (uint64_t)s.I * es;   // row strides in bytes
   {
-    const uint64_t dims[3] = {(uint64_t)s.H, (uint64_t)s.I, (uint64_t)a->nslots};
-    const uint64_t str[2] = {(uint64_t)s.H * es, (uint64_t)a->slot_bytes};
+    const uint64_t dims[3] = {kH, (uint64_t)s.I, (uint64_t)a->nslots};
+    const uint64_t str[2] = {rH, (uint64_t)a->slot_bytes};
     int r = encode_map(c, tg, dt, a->base + s.off_gate, 3, dims, str, box);
     if (r) return r;
     r = encode_map(c, tu, dt, a->base + s.off_up, 3, dims, str, box);
     if (r) return r;
   }
   {
-    const uint64_t dims[3] = {(uint64_t)s.I, (uint64_t)s.H, (uint64_t)a->nslots};
-    const uint64_t str[2] = {(uint64_t)s.I * es, (uint64_t)a->slot_bytes};
+    const uint64_t dims[3] = {kI, (uint64_t)s.H, (uint64_t)a->nslots};
+    const uint64_t str[2] = {rI, (uint64_t)a->slot_bytes};
     int r = encode_map(c, td, dt, a->base + s.off_down, 3, dims, str, box);
     if (r) return r;
   }
@@ -738,9 +762,10 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (!cfg || !out) return fail(nullptr, B2M_EINVAL, "null argument");
   if (cfg->struct_size != (int)sizeof(b2m_config))
     return fail(nullptr, B2M_EINVAL, "b2m_config size mismatch (%d vs %d)", cfg->struct_size, (int)sizeof(b2m_config));
-  if (weight_format != B2M_WEIGHTS_MODEL_DTYPE && weight_format != B2M_WEIGHTS_FP8_E4M3_B128)
+  if (weight_format != B2M_WEIGHTS_MODEL_DTYPE && weight_format != B2M_WEIGHTS_FP8_E4M3_B128 &&
+      weight_format != B2M_WEIGHTS_INT4_G128)
     return fail(nullptr, B2M_EINVAL, "unknown weight format %d", weight_format);
-  const bool fp8 = weight_format == B2M_WEIGHTS_FP8_E4M3_B128;
+  const bool fp8 = weight_format == B2M_WEIGHTS_FP8_E4M3_B128, int4 = weight_format == B2M_WEIGHTS_INT4_G128;
   if (cfg->dtype == B2M_DTYPE_FP8_E4M3)
     return fail(nullptr, B2M_EUNSUPPORTED, "dtype %d (fp8): the reference's own torch::matmul has no Float8 kernel; bf16, f16 and f32 experts are supported", cfg->dtype);
   if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16 && cfg->dtype != B2M_DTYPE_F32) return fail(nullptr, B2M_EINVAL, "bad dtype");
@@ -750,7 +775,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       cfg->max_tokens < 1)
     return fail(nullptr, B2M_EINVAL, "bad model dimensions");
   ExpertShape shape;
-  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, &shape, fp8 ? 1 : esize))
+  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, &shape, fp8 || int4 ? 1 : esize))
     return fail(nullptr, B2M_EUNSUPPORTED, "expert_type %d is unknown (expert_module.h:13-18 defines 0..5)", cfg->expert_type);
   if (fp8) {
     if (cfg->dtype != B2M_DTYPE_BF16)
@@ -763,6 +788,18 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
     if (cfg->gemm_impl == 1)
       return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
     make_fp8_shape(&shape);
+  }
+  if (int4) {
+    if (cfg->dtype != B2M_DTYPE_BF16)
+      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights need a bf16 model dtype (activations), got dtype %d", cfg->dtype);
+    if (cfg->expert_type != B2M_EXPERT_MIXTRAL_MOE_DENSE_ACT_DENSE && cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
+      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights support Mixtral (4) and DeepSeek (5) experts, got expert_type %d", cfg->expert_type);
+    if (cfg->hidden % i4::GROUP || cfg->inter % i4::GROUP)
+      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights need hidden and inter to be multiples of %d (128-input groups, 128-row tiles), got %d / %d",
+                  i4::GROUP, cfg->hidden, cfg->inter);
+    if (cfg->gemm_impl == 1)
+      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
+    make_int4_shape(&shape);
   }
   if (cfg->router < 0 || cfg->router > 4) return fail(nullptr, B2M_EINVAL, "bad router kind");
   if (cfg->router == B2M_ROUTER_DEEPSEEK_V3) {
@@ -789,6 +826,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (!c) return fail(nullptr, B2M_ENOMEM, "out of host memory");
   c->cfg = *cfg;
   c->fp8 = fp8;
+  c->int4 = int4;
   memset(&c->stats, 0, sizeof c->stats);
 #define CKC(call)                                                                                     \
   do {                                                                                                \
@@ -834,7 +872,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   c->offload = nslots < (long long)L * E;
   CKC(cudaMalloc((void**)&c->arena.base, (size_t)nslots * shape.bytes));
   c->arena.owned = true;
-  for (int m = 0; m < 3 && !fp8; ++m) {   // (an fp8 context has no 12-bit packed copy: pk.slot_bytes stays 0)
+  for (int m = 0; m < 3 && !fp8 && !int4; ++m) {   // (an fp8 / int4 context has no 12-bit packed copy: pk.slot_bytes stays 0)
     c->pk.off[m] = c->pk.slot_bytes;
     c->pk.slot_bytes += packed_matrix_bytes((int)pk_matrix_rows(shape, m), (int)pk_matrix_cols(shape, m));
   }
@@ -1261,6 +1299,12 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
       up.f8_s1 = a.base + s.sc_up;
       dn.f8_s0 = dn.f8_s1 = a.base + s.sc_down;
       up.f8_slot_bytes = dn.f8_slot_bytes = a.slot_bytes;
+    }
+    if (&a == &c->arena && s.int4) {
+      up.i4_g0 = a.base + s.sc_gate;
+      up.i4_g1 = a.base + s.sc_up;
+      dn.i4_g0 = dn.i4_g1 = a.base + s.sc_down;
+      up.i4_slot_bytes = dn.i4_slot_bytes = a.slot_bytes;
     }
     if (&a == &c->arena && c->pk.state == 1) {
       up.pk_ok = dn.pk_ok = c->pk.d_ok;
@@ -1776,6 +1820,7 @@ static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (!c) return B2M_EINVAL;
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
   if (c->fp8) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with fp8 weights");
+  if (c->int4) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with int4 weights");
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
     return fail(c, B2M_EINVAL, "bad expert-parallel geometry (nranks=%d rank=%d cap=%d E=%d)", nranks, rank, cap, c->cfg.num_experts);
   if ((long long)nranks * cap > c->cap_R)

@@ -26,6 +26,7 @@
 #include "ep_device.cuh"
 #include "tile_walker.cuh"
 #include "fp8_weights.cuh"
+#include "int4_weights.cuh"
 #include "weight_pack.cuh"
 
 namespace b2m {
@@ -40,11 +41,12 @@ constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on s
 // Where a GEMM's A operand (the weight tile) comes from
 enum : int { AS_BF16 = 0,   // bf16 tile in shared memory, read by the wgmma itself
              AS_PK12 = 1,   // bf16 tile or 12-bit packed record (weight_pack.cuh), decoded into register fragments
-             AS_FP8 = 2 };  // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
+             AS_FP8 = 2,    // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
+             AS_INT4 = 3 }; // 4-bit code tile + per-128-input scale / zero point (int4_weights.cuh), dequantised likewise
 
 template <int NT, bool DUAL, int AS = AS_BF16>
 struct GemmCfg {
-  static constexpr int A_BYTES = AS == AS_FP8 ? f8::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
+  static constexpr int A_BYTES = AS == AS_FP8 ? f8::TILE_BYTES : AS == AS_INT4 ? i4::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
   static constexpr int B_TILE_BYTES = NT * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_BYTES + B_TILE_BYTES;
   static constexpr int STAGES_RAW = SMEM_BUDGET / STAGE_BYTES;
@@ -72,6 +74,7 @@ struct GemmCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "over the sm_90 shared-memory limit");
   static_assert(wp::REC_BYTES <= A_TILE_BYTES && wp::ROWS == BLOCK_M && wp::COLS == BLOCK_K, "a packed record fills an A slot of the stage");
   static_assert(f8::ROWS == BLOCK_M && f8::COLS == BLOCK_K && A_BYTES % 1024 == 0, "an fp8 tile keeps the stage's 1024-B alignment");
+  static_assert(i4::ROWS == BLOCK_M && i4::COLS == BLOCK_K && i4::GROUP == 2 * BLOCK_K, "an int4 tile is one k-block, a group two");
 };
 
 __device__ __forceinline__ float act_apply(float x, int act) {
@@ -131,11 +134,14 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
 // FP8 (AS_FP8: bf16, MC == 1, no m_rows / expert-parallel regions; every tile width): the A maps are uint8 maps over e4m3
 // matrices; the producer loads 8-KiB e4m3 tiles and the consumers dequantise their fragments with the tile's block scale
 // (fp8_weights.cuh) into the same register-A wgmmas, over the same tile walk and launch plan as the bf16 engine.
+// INT4 (AS_INT4: same restrictions and plan as FP8): the A maps are uint8 maps over the 4-bit code matrices (32-byte rows);
+// the producer loads 4-KiB code tiles and the consumers dequantise their fragments with the group words of their rows
+// (int4_weights.cuh), read from the tile-major group grids one k-block ahead.
 template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, int AS = AS_BF16>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
                                           const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
   using Cfg = GemmCfg<NT, DUAL, AS>;
-  constexpr bool PK = AS == AS_PK12, F8 = AS == AS_FP8;
+  constexpr bool PK = AS == AS_PK12, F8 = AS == AS_FP8, I4 = AS == AS_INT4;
   constexpr int A_BYTES = Cfg::A_BYTES;
   // carve shared memory: [stages | barriers | tile tables]
   uint8_t* stage_base = smem;
@@ -149,6 +155,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   int* pkf = cnts + MAX_E;             // PK: pk_ok of each expert's slot
   static_assert(!PK || (MC == 1 && DT == DT_BF16 && NT <= 64), "packed weights: bf16 decode-sized tiles");
   static_assert(!F8 || (MC == 1 && DT == DT_BF16), "fp8 weights: bf16 activations, single-CTA tiles");
+  static_assert(!I4 || (MC == 1 && DT == DT_BF16), "int4 weights: bf16 activations, single-CTA tiles");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -274,7 +281,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
           uint8_t* sA0 = stage_base + stage * Cfg::STAGE_BYTES;
           uint8_t* sA1 = sA0 + A_BYTES;
           uint8_t* sB = sA0 + (DUAL ? 2 : 1) * A_BYTES;
-          const int a_bytes = m_rows * BLOCK_K * (F8 ? 1 : 2);
+          const int a_bytes = I4 ? m_rows * i4::ROW_BYTES : m_rows * BLOCK_K * (F8 ? 1 : 2);
           mbar_arrive_expect_tx(&full_bar[stage], (DUAL ? 2 : 1) * (pk0 ? wp::REC_BYTES : a_bytes) + Cfg::B_TILE_BYTES);
           // decode: weights are streamed exactly once -> evict-first.  Several n-tiles per expert (prefill): the same
           // weight tile is re-read by every n-tile -> keep it in L2.  Tokens are re-read by every m-tile: keep.
@@ -284,8 +291,11 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
               bulk_load(&full_bar[stage], sA0, rec + (size_t)kb * wp::REC_BYTES, wp::REC_BYTES, wh);
               if (DUAL) bulk_load(&full_bar[stage], sA1, rec + (p.pk_a1 - p.pk_a0) + (size_t)kb * wp::REC_BYTES, wp::REC_BYTES, wh);
             } else {
-              tma_load_3d(&tmA0, &full_bar[stage], sA0, kb * BLOCK_K, t.m0, t.slot, wh);
-              if (DUAL) tma_load_3d(&tmA1, &full_bar[stage], sA1, kb * BLOCK_K, t.m0 + (p.dual_m ? BLOCK_M : 0), t.slot, wh);
+              // (k coordinate of the A maps: int4 maps count bytes, two codes each)
+              tma_load_3d(&tmA0, &full_bar[stage], sA0, I4 ? kb * i4::ROW_BYTES : kb * BLOCK_K, t.m0, t.slot, wh);
+              if (DUAL)
+                tma_load_3d(&tmA1, &full_bar[stage], sA1, I4 ? kb * i4::ROW_BYTES : kb * BLOCK_K, t.m0 + (p.dual_m ? BLOCK_M : 0),
+                            t.slot, wh);
             }
           } else {
             // 2-CTA multicast: the cluster's CTAs work on the same weight tiles and adjacent token tiles; each CTA fetches
@@ -353,8 +363,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
     // k-block is decoded into the other (wgmma_wait<1> retires the older one).  The fp8 DUAL 128-token tile keeps ONE buffer:
     // beside its 128 accumulator registers a second one spills.  Its decode then waits for the previous k-block's wgmmas; the
     // other consumer warpgroup's wgmmas keep the tensor cores busy meanwhile (this width only runs at prefill).
-    constexpr int FRAG_BUFS = (F8 && DUAL && NT == 128) ? 1 : 2;
-    uint32_t fa0[FRAG_BUFS][16], fa1[FRAG_BUFS][16];   // (unused without PK / F8)
+    constexpr int FRAG_BUFS = ((F8 || I4) && DUAL && NT == 128) ? 1 : 2;
+    uint32_t fa0[FRAG_BUFS][16], fa1[FRAG_BUFS][16];   // (unused without PK / F8 / I4)
     for (int tile = tile0; walker.get(tile, t); tile += tile_stride) {
       int prev = -1;
       auto next_stage = [&]() {
@@ -393,6 +403,31 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         sn0 = __ldg(sc0 + t.kb_begin / 2);
         if (DUAL) sn1 = __ldg(sc1 + t.kb_begin / 2);
       }
+      // INT4: group words of this thread's rows ra, ra + 8 in A0 / A1 (tile-major grids: the 128 rows of a tile's group are
+      // contiguous; dual_m as for FP8).  One word per row and 128 k, loaded one k-block ahead of its use.
+      struct I4Groups {
+        const uint32_t* w[2];   // A0 / A1: word of row ra in group 0 of the tile
+        uint32_t cur[2][2];     // [A0 / A1][row ra / ra + 8]: words of the k-block being decoded ...
+        uint32_t nxt[2][2];     // ... and of the next one
+        __device__ __forceinline__ void load(int kb) {
+          const int g = kb / 2;
+#pragma unroll
+          for (int a = 0; a < (DUAL ? 2 : 1); ++a) {
+            nxt[a][0] = __ldg(w[a] + g * BLOCK_M);
+            nxt[a][1] = __ldg(w[a] + g * BLOCK_M + 8);
+          }
+        }
+      };
+      struct NoGroups {};
+      std::conditional_t<I4, I4Groups, NoGroups> grp;
+      if constexpr (I4) {
+        const int gs = p.K / i4::GROUP, mt = t.m0 / BLOCK_M, mts = p.M / BLOCK_M;
+        grp.w[0] = reinterpret_cast<const uint32_t*>(p.i4_g0 + (size_t)t.slot * p.i4_slot_bytes) + (size_t)mt * gs * BLOCK_M + ra;
+        grp.w[1] = DUAL ? reinterpret_cast<const uint32_t*>(p.i4_g1 + (size_t)t.slot * p.i4_slot_bytes) +
+                              (size_t)(p.dual_m && mt + 1 < mts ? mt + 1 : mt) * gs * BLOCK_M + ra
+                        : grp.w[0];
+        grp.load(t.kb_begin);
+      }
       // one k-block, A decoded from packed records / dequantised from e4m3 into fragment buffer BUF (compile time)
       auto kblock_packed = [&](int kb, auto BUF) {
         constexpr int bf = decltype(BUF)::value;
@@ -405,12 +440,20 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
             if (DUAL) sn1 = __ldg(sc1 + (kb + 1) / 2);
           }
         }
+        if constexpr (I4) {
+#pragma unroll
+          for (int a = 0; a < 2; ++a) { grp.cur[a][0] = grp.nxt[a][0]; grp.cur[a][1] = grp.nxt[a][1]; }
+          if (kb + 1 < t.kb_end) grp.load(kb + 1);
+        }
         mbar_wait(&full_bar[stage], phase);
         if constexpr (FRAG_BUFS == 1) wgmma_wait<0>();   // the previous k-block's wgmmas have read the fragments
         const uint8_t* sa = stage_base + stage * Cfg::STAGE_BYTES;
         if constexpr (F8) {
           f8::decode_lane(sa, ct, s0, fa0[bf]);
           if constexpr (DUAL) f8::decode_lane(sa + A_BYTES, ct, s1, fa1[bf]);
+        } else if constexpr (I4) {
+          i4::decode_lane(sa, ct, grp.cur[0][0], grp.cur[0][1], fa0[bf]);
+          if constexpr (DUAL) i4::decode_lane(sa + A_BYTES, ct, grp.cur[1][0], grp.cur[1][1], fa1[bf]);
         } else {
           wp::decode_lane(sa, ct, fa0[bf]);
           if constexpr (DUAL) wp::decode_lane(sa + A_BYTES, ct, fa1[bf]);
@@ -430,12 +473,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         next_stage();
       };
       // a tile streams packed records when every A matrix it reads has a current packed copy (the producer decides the same)
-      bool packed = F8;
+      bool packed = F8 || I4;
       if constexpr (PK) packed = ((pkf[t.e] >> p.pk_bit0) & 1) && (!DUAL || ((pkf[t.e] >> p.pk_bit1) & 1));
       if (!packed) {
-        if constexpr (!F8)
+        if constexpr (!F8 && !I4)
           for (int kb = t.kb_begin; kb < t.kb_end; ++kb) kblock_smem(kb);
-      } else if constexpr (PK || F8) {
+      } else if constexpr (PK || F8 || I4) {
         for (int kb = t.kb_begin; kb < t.kb_end; ++kb) {
           kblock_packed(kb, std::integral_constant<int, 0>{});
           if (++kb >= t.kb_end) break;
@@ -722,6 +765,25 @@ cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& g, const CUte
 template <int DT>
 static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
                                const GemmParams& p, int grid, cudaStream_t st) {
+  // int4 weights: every tile width the bf16 plan picks, same plan (the caller's p)
+  if constexpr (DT == DT_BF16) {
+    if (p.i4_g0) {
+#define B2M_ICASE(N)                                                                \
+  case N:                                                                           \
+    return dual ? launch_tc<N, true, DT, 1, AS_INT4>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
+      switch (nt) {
+        B2M_ICASE(16)
+        B2M_ICASE(32)
+        B2M_ICASE(64)
+        B2M_ICASE(128)
+        case 256:
+          return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
+        default:
+          return cudaErrorInvalidValue;
+      }
+#undef B2M_ICASE
+    }
+  }
   // fp8 weights: every tile width the bf16 plan picks, same plan (the caller's p)
   if constexpr (DT == DT_BF16) {
     if (p.f8_s0) {
@@ -923,7 +985,7 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
     return launch_grouped_gemm_tc(dtype, nt, dual, a0, a1, b, q, grid, st);
   }
   if (dtype == DT_BF16) return dispatch_nt<DT_BF16>(nt, dual, a0, a1, b, p, grid, st);
-  if (dtype == DT_F16 && !p.f8_s0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
+  if (dtype == DT_F16 && !p.f8_s0 && !p.i4_g0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
   return cudaErrorInvalidValue;
 }
 

@@ -9,8 +9,8 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(os.path.dirname(PKG_DIR), "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libb2m.so")
 SOURCES = ["grouped_gemm.cu", "route.cu", "ep.cu", "f32_path.cu", "tracer.cu", "store_reader.cpp", "api.cu"]
-HEADERS = ["b2m_common.cuh", "b2m_internal.h", "tile_walker.cuh", "weight_pack.cuh", "fp8_weights.cuh", "ep_device.cuh",
-           os.path.join("..", "..", "include", "b2m.h")]
+HEADERS = ["b2m_common.cuh", "b2m_internal.h", "tile_walker.cuh", "weight_pack.cuh", "fp8_weights.cuh", "int4_weights.cuh",
+           "ep_device.cuh", os.path.join("..", "..", "include", "b2m.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 OBJ_DIR = os.path.join(CSRC, "_obj")     # git-ignored (*.o); one object per translation unit, compiled in parallel

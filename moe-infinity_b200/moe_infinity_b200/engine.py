@@ -14,6 +14,7 @@ import torch
 
 from . import _lib as L
 from . import fp8 as F8
+from . import int4 as I4
 
 _TORCH2INT = {torch.bfloat16: L.DTYPE_BF16, torch.float32: L.DTYPE_F32, torch.float16: L.DTYPE_F16}
 _INT2TORCH = {v: k for k, v in _TORCH2INT.items()}
@@ -51,17 +52,22 @@ class MoEEngine:
                  pack_weights: bool = True, expert_dtype: Optional[torch.dtype] = None):
         """expert_dtype: None = the routed experts are stored in `dtype`; torch.float8_e4m3fn = FP8 E4M3 with one fp32 scale
         per 128x128 block (`fp8.py`; `dtype` stays the activation dtype and must be bf16; register_expert / load_expert then
-        take the three e4m3 matrices and their scale grids)."""
+        take the three e4m3 matrices and their scale grids); torch.uint4 = 4-bit codes with a bf16 scale and a 4-bit zero
+        point per 128 inputs (`int4.py`; `dtype` must be bf16; register_expert / load_expert then take the three packed code
+        matrices with scales= and zeros=)."""
         self.lib = L.load()
         if not torch.cuda.is_available():
             raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if dtype not in _TORCH2INT:
             raise ValueError(f"unsupported dtype {dtype}")
-        if expert_dtype is not None and expert_dtype != torch.float8_e4m3fn:
-            raise ValueError(f"unsupported expert_dtype {expert_dtype} (None or torch.float8_e4m3fn)")
-        self.fp8 = expert_dtype is not None
+        if expert_dtype is not None and expert_dtype not in (torch.float8_e4m3fn, torch.uint4):
+            raise ValueError(f"unsupported expert_dtype {expert_dtype} (None, torch.float8_e4m3fn or torch.uint4)")
+        self.fp8 = expert_dtype == torch.float8_e4m3fn
+        self.int4 = expert_dtype == torch.uint4
         if self.fp8 and dtype != torch.bfloat16:
             raise ValueError("fp8 experts compute with bf16 activations: dtype must be torch.bfloat16")
+        if self.int4 and dtype != torch.bfloat16:
+            raise ValueError("int4 experts compute with bf16 activations: dtype must be torch.bfloat16")
         self.dtype = dtype
         self.device = torch.device("cuda", device)
         self.L, self.E, self.H, self.I, self.k = num_layers, num_experts, hidden, inter, top_k
@@ -93,7 +99,7 @@ class MoEEngine:
         self.max_tokens = max_tokens
         h = C.c_void_p()
         torch.cuda.set_device(self.device)
-        fmt = L.WEIGHTS_FP8_E4M3_B128 if self.fp8 else L.WEIGHTS_MODEL_DTYPE
+        fmt = L.WEIGHTS_FP8_E4M3_B128 if self.fp8 else L.WEIGHTS_INT4_G128 if self.int4 else L.WEIGHTS_MODEL_DTYPE
         L.check(None, self.lib.b2m_ctx_create_ex(C.byref(cfg), fmt, C.byref(h)))
         self._h = h
         self._blobs: Dict[Tuple[int, int], torch.Tensor] = {}
@@ -107,6 +113,8 @@ class MoEEngine:
             self.expert_bytes = nmat * hidden * inter * es
         if self.fp8:
             self.expert_bytes = F8.expert_blob_bytes(hidden, inter)
+        if self.int4:
+            self.expert_bytes = I4.expert_blob_bytes(hidden, inter)
         self.shared_bytes = 3 * hidden * shared_inter * es
 
     # ------------------------------------------------------------------ lifecycle
@@ -160,19 +168,56 @@ class MoEEngine:
             parts.append(s.detach().contiguous().view(torch.uint8).reshape(-1))
         return parts
 
+    def _int4_parts(self, tensors: Sequence[torch.Tensor], scales: Optional[Sequence[torch.Tensor]],
+                    zeros: Optional[Sequence[torch.Tensor]]) -> List[torch.Tensor]:
+        """The int4 expert blob's parts as flat uint8 tensors: three packed code matrices, then their tile-major group
+        grids (int4.py)."""
+        if scales is None or zeros is None:
+            raise ValueError("an int4 engine needs the three scale and zero-point grids: scales=(s1, s2, s3), zeros=(z1, z2, z3)")
+        if len(tensors) != 3 or len(scales) != 3 or len(zeros) != 3:
+            raise ValueError("an int4 expert is three code matrices, three scale grids and three zero-point grids")
+        H, I = self.H, self.I
+        # nn.Linear [out, in]: Mixtral w1 | w2 | w3 = gate, down, up; DeepSeek gate | up | down
+        shapes = [(I, H), (H, I), (I, H)] if self.expert_type == L.EXPERT_MIXTRAL else [(I, H), (I, H), (H, I)]
+        parts, grids = [], []
+        for t, s, z, (r, c) in zip(tensors, scales, zeros, shapes):
+            if t.dtype != torch.uint8 or tuple(t.shape) != (r, c // 2):
+                raise ValueError(f"expected a uint8 {(r, c // 2)} code matrix (two codes per byte), got {t.dtype} {tuple(t.shape)}")
+            want = (r, c // I4.GROUP)
+            if s.dtype != torch.bfloat16 or tuple(s.shape) != want:
+                raise ValueError(f"expected a bfloat16 {want} scale grid, got {s.dtype} {tuple(s.shape)}")
+            if z.dtype != torch.uint8 or tuple(z.shape) != want:
+                raise ValueError(f"expected a uint8 {want} zero-point grid, got {z.dtype} {tuple(z.shape)}")
+            parts.append(t.detach().contiguous().reshape(-1))
+            grids.append(I4.pack_groups(s.detach(), z.detach().to(s.device)))
+        return parts + grids
+
+    def _quant_parts(self, tensors, scales, zeros) -> Optional[List[torch.Tensor]]:
+        """The blob parts of a quantised engine's expert; None on a model-dtype engine (which takes no scales / zeros)."""
+        if self.fp8:
+            if zeros is not None:
+                raise ValueError("zeros go with the int4 codes of an int4 engine (expert_dtype=torch.uint4)")
+            return self._fp8_parts(tensors, scales)
+        if self.int4:
+            return self._int4_parts(tensors, scales, zeros)
+        if scales is not None or zeros is not None:
+            raise ValueError("scales / zeros are only taken by an fp8 or int4 engine (expert_dtype=torch.float8_e4m3fn / torch.uint4)")
+        return None
+
     def register_expert(self, layer: int, expert: int, tensors: Sequence[torch.Tensor], pin: bool = True,
-                        scales: Optional[Sequence[torch.Tensor]] = None):
+                        scales: Optional[Sequence[torch.Tensor]] = None, zeros: Optional[Sequence[torch.Tensor]] = None):
         """Host-backed expert (can be staged in and evicted).  tensors: Mixtral (w1,w2,w3),
         DeepSeek (gate,up,down), Switch (wi,wo), NLLB/FSGPT (fc1,fc1_bias,fc2,fc2_bias) -- nn.Linear [out,in] layout.
-        fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids."""
-        if self.fp8:
+        fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids.
+        int4 engine: the three uint8 [out, in/2] code matrices (int4.quantize_g128), `scales` (bfloat16 [out, in/128]) and
+        `zeros` (uint8 [out, in/128])."""
+        parts = self._quant_parts(tensors, scales, zeros)
+        if parts is not None:
             blob = torch.zeros(self.expert_bytes, dtype=torch.uint8, pin_memory=pin)
             off = 0
-            for part in self._fp8_parts(tensors, scales):
+            for part in parts:
                 blob[off:off + part.numel()] = part.cpu()
                 off += part.numel()
-        elif scales is not None:
-            raise ValueError("scales are only taken by an fp8 engine (expert_dtype=torch.float8_e4m3fn)")
         else:
             blob = self._pack(tensors, self.expert_bytes, pin)
         self._blobs[(layer, expert)] = blob
@@ -196,24 +241,26 @@ class MoEEngine:
         self._ck(self.lib.b2m_expert_dev_ptr(self._h, layer, expert, C.byref(p)))
         if not p.value:
             return None
-        if self.fp8:   # the fp8 expert blob (fp8.py): e4m3 matrices, then fp32 scale grids
+        if self.fp8 or self.int4:   # the fp8 / int4 expert blob (fp8.py / int4.py): quantised matrices, then their grids
             return _view(p.value, (self.expert_bytes,), torch.uint8, self.device)
         return _view(p.value, (self.expert_bytes // self.esize,), self.dtype, self.device)
 
     def load_expert(self, layer: int, expert: int, tensors: Optional[Sequence[torch.Tensor]] = None,
-                    scales: Optional[Sequence[torch.Tensor]] = None):
+                    scales: Optional[Sequence[torch.Tensor]] = None, zeros: Optional[Sequence[torch.Tensor]] = None):
         """HBM-only expert: claims a slot, pins it, fills it from `tensors` (any device) if given.
         Returns the flat device view of the slot so callers can initialise it in place.  Writes through the view must be
         issued (on the current stream) before the next forward of this layer; the second eager forward after the load packs
         the slot for the decode GEMMs (pack_weights=True); to change the weights later, call load_expert again and write through the view it returns.
-        fp8 engine: `tensors` are the three float8_e4m3fn matrices and `scales` their float32 grids; the view is uint8."""
-        if self.fp8 and tensors is not None:
-            parts = self._fp8_parts(tensors, scales)
-        elif scales is not None:
-            raise ValueError("scales go with the fp8 matrices of an fp8 engine")
+        fp8 engine: `tensors` are the three float8_e4m3fn matrices and `scales` their float32 grids; the view is uint8.
+        int4 engine: `tensors` are the three uint8 code matrices, `scales` / `zeros` their bf16 / uint8 grids; the view is uint8."""
+        parts = None
+        if tensors is not None:
+            parts = self._quant_parts(tensors, scales, zeros)
+        elif scales is not None or zeros is not None:
+            raise ValueError("scales / zeros go with the quantised matrices of an fp8 or int4 engine")
         self._ck(self.lib.b2m_make_resident(self._h, layer, expert, 1 | 2, C.c_void_p(_stream_ptr())))
         v = self.expert_device_view(layer, expert)
-        if self.fp8 and tensors is not None:
+        if parts is not None:
             off = 0
             for part in parts:
                 v[off:off + part.numel()].copy_(part)

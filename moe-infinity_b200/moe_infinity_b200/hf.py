@@ -17,7 +17,24 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from . import fp8 as F8
+from . import int4 as I4
 from .engine import MoEEngine
+
+
+def _load(engine: MoEEngine, layer: int, expert: int, ws, resident: bool):
+    """Hand one expert's bf16 matrices to `engine`, quantised first when the engine stores fp8 (`fp8.quantize_block128`) or
+    int4 (`int4.quantize_g128`) experts."""
+    kw = {}
+    if engine.fp8:
+        ws, scales = zip(*[F8.quantize_block128(w) for w in ws])
+        kw = dict(scales=scales)
+    elif engine.int4:
+        ws, scales, zeros = zip(*[I4.quantize_g128(w) for w in ws])
+        kw = dict(scales=scales, zeros=zeros)
+    if resident:
+        engine.load_expert(layer, expert, ws, **kw)
+    else:
+        engine.register_expert(layer, expert, ws, **kw)
 
 
 class B200MixtralMoeAdapter(nn.Module):
@@ -41,7 +58,8 @@ def patch_mixtral(model, max_tokens: int = 4096, num_slots: int = 0, device_memo
                   resident: bool = True, engine: Optional[MoEEngine] = None) -> MoEEngine:
     """Move every expert of `model` (a transformers MixtralForCausalLM / MixtralModel on a CUDA device) into a
     MoEEngine and replace the MoE blocks.  `resident=False` registers experts as pinned host blobs (offload mode,
-    budget from num_slots / device_memory_ratio) instead of loading all of them into HBM."""
+    budget from num_slots / device_memory_ratio) instead of loading all of them into HBM.  `engine` may be given (built with
+    the model's shapes), e.g. one with expert_dtype=torch.uint4: the experts are then quantised with `int4.quantize_g128`."""
     cfg = model.config
     layers = model.model.layers if hasattr(model, "model") else model.layers
     dev = next(model.parameters()).device
@@ -56,10 +74,7 @@ def patch_mixtral(model, max_tokens: int = 4096, num_slots: int = 0, device_memo
         gu, dn = moe.experts.gate_up_proj.data, moe.experts.down_proj.data     # [E,2I,H], [E,H,I]
         for e in range(E):
             w1, w3, w2 = gu[e, :I], gu[e, I:], dn[e]                            # reference order: w1 | w2 | w3
-            if resident:
-                engine.load_expert(l, e, [w1, w2, w3])
-            else:
-                engine.register_expert(l, e, [w1, w2, w3])
+            _load(engine, l, e, [w1, w2, w3], resident)
         layer.mlp = B200MixtralMoeAdapter(engine, l, moe.gate.weight.data)
     return engine
 
@@ -85,8 +100,8 @@ def patch_deepseek_v3(model, max_tokens: int = 4096, num_slots: int = 0, device_
     """Move the routed experts, shared experts, router weights and correction biases of `model` (a transformers
     DeepseekV3ForCausalLM / DeepseekV3Model on a CUDA device) into a MoEEngine (ROUTER_DEEPSEEK_V3) and replace its MoE
     blocks (layers >= config.first_k_dense_replace; the dense layers before them stay as they are).  `engine` may be
-    given (built with router=ROUTER_DEEPSEEK_V3 and the model's shapes), e.g. one with expert_dtype=torch.float8_e4m3fn:
-    the experts are then quantised with `fp8.quantize_block128`.  `resident=False` registers experts as pinned host
+    given (built with router=ROUTER_DEEPSEEK_V3 and the model's shapes), e.g. one with expert_dtype=torch.float8_e4m3fn or
+    torch.uint4: the experts are then quantised with `fp8.quantize_block128` or `int4.quantize_g128`.  `resident=False` registers experts as pinned host
     blobs (offload mode, budget from num_slots / device_memory_ratio)."""
     cfg = model.config
     if cfg.num_experts_per_tok == 1 and cfg.norm_topk_prob:
@@ -109,13 +124,7 @@ def patch_deepseek_v3(model, max_tokens: int = 4096, num_slots: int = 0, device_
         moe = layers[l].mlp
         gu, dn = moe.experts.gate_up_proj.data, moe.experts.down_proj.data     # [E,2I,H], [E,H,I]
         for e in range(E):
-            ws, scales = [gu[e, :I], gu[e, I:], dn[e]], None                   # DeepSeek order: gate | up | down
-            if engine.fp8:
-                ws, scales = zip(*[F8.quantize_block128(w) for w in ws])
-            if resident:
-                engine.load_expert(l, e, ws, scales=scales)
-            else:
-                engine.register_expert(l, e, ws, scales=scales)
+            _load(engine, l, e, [gu[e, :I], gu[e, I:], dn[e]], resident)     # DeepSeek order: gate | up | down
         sh = moe.shared_experts
         engine.register_shared(l, [sh.gate_proj.weight.data, sh.up_proj.weight.data, sh.down_proj.weight.data])
         engine.set_gate(l, moe.gate.weight.data)
