@@ -204,6 +204,22 @@ int b2m_ctx_destroy(b2m_ctx* ctx);
                                        ((r/128) * (cols/128) + g) * 128 + r%128.  Activations, outputs, workspaces and the
                                        router stay bf16; DeepSeek shared experts stay bf16.  Restrictions (B2M_EUNSUPPORTED
                                        with a message) and the expert-parallel refusal: as B2M_WEIGHTS_FP8_E4M3_B128. */
+/* (5 is not a weight format: B2M_EINVAL) */
+#define B2M_WEIGHTS_INT4_G128_F16 6 /* B2M_WEIGHTS_INT4_G128 with fp16 scales and f16 activations: the format of AWQ and GPTQ
+                                       4-bit checkpoints (group size 128).  Each routed matrix is codes q[r][c] in 0..15,
+                                       scales s[r][c/128] (fp16) and zero points z[r][c/128] in 0..15.  The experts compute
+                                       exactly what the f16 engine computes on
+                                         W[r][c] = f16(s[r][c/128] * (q[r][c] - z[r][c/128]))
+                                       -- the product is exact in fp32 and is rounded once to nearest-even, subnormals kept,
+                                       overflow to +-Inf (torch: `(s_expanded.float() * (q.float() -
+                                       z_expanded.float())).to(torch.float16)`); this is the value AWQ's and GPTQ's own
+                                       dequantisation produces.  Expert blob: byte for byte the layout of
+                                       B2M_WEIGHTS_INT4_G128 (same size and offsets), except that bits 0..15 of each group word
+                                       are the fp16 bits of s.  Activations, outputs, workspaces and the router are f16;
+                                       DeepSeek shared experts stay f16.  Restrictions, each refused by b2m_ctx_create_ex with
+                                       B2M_EUNSUPPORTED and a message: cfg.dtype f16; expert types Mixtral (4) and DeepSeek
+                                       (5); hidden and inter multiples of 128; gemm_impl 0 or 2.  The expert-parallel entry
+                                       points return B2M_EUNSUPPORTED on such a context. */
 /* b2m_ctx_create with the routed experts stored in `weight_format` (B2M_WEIGHTS_*; any other value: B2M_EINVAL) */
 int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out);
 

@@ -185,7 +185,7 @@ struct b2m_ctx {
 
   int cur_ksplit = 1, cur_nt = 16, cur_nt_dn = 16, cur_T = 0;   // token-tile widths of the up (K3) and down (K4) GEMMs
   bool fp8 = false;           // routed experts in B2M_WEIGHTS_FP8_E4M3_B128 (arena.shape.fp8)
-  bool int4 = false;          // routed experts in B2M_WEIGHTS_INT4_G128 (arena.shape.int4)
+  bool int4 = false;          // routed experts in B2M_WEIGHTS_INT4_G128 or _F16 (arena.shape.int4; the scales' type is cfg.dtype)
   bool ep_mode = false;       // experts of other ranks are simply absent (never an error)
   // 12-bit packed copy of the routed arena (weight_pack.cuh; same slot index), read by the decode GEMMs.  Allocated by the first
   // eager forward that packs, if the device keeps PK_RESERVE free beside it.  d_ok[slot]: bit b = matrix b (gate, up, down)
@@ -763,9 +763,11 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (cfg->struct_size != (int)sizeof(b2m_config))
     return fail(nullptr, B2M_EINVAL, "b2m_config size mismatch (%d vs %d)", cfg->struct_size, (int)sizeof(b2m_config));
   if (weight_format != B2M_WEIGHTS_MODEL_DTYPE && weight_format != B2M_WEIGHTS_FP8_E4M3_B128 &&
-      weight_format != B2M_WEIGHTS_INT4_G128)
+      weight_format != B2M_WEIGHTS_INT4_G128 && weight_format != B2M_WEIGHTS_INT4_G128_F16)
     return fail(nullptr, B2M_EINVAL, "unknown weight format %d", weight_format);
-  const bool fp8 = weight_format == B2M_WEIGHTS_FP8_E4M3_B128, int4 = weight_format == B2M_WEIGHTS_INT4_G128;
+  // (the two int4 formats share the slot layout; their group scales are of the activations' type, bf16 or f16)
+  const bool fp8 = weight_format == B2M_WEIGHTS_FP8_E4M3_B128, int4_f16 = weight_format == B2M_WEIGHTS_INT4_G128_F16,
+             int4 = weight_format == B2M_WEIGHTS_INT4_G128 || int4_f16;
   if (cfg->dtype == B2M_DTYPE_FP8_E4M3)
     return fail(nullptr, B2M_EUNSUPPORTED, "dtype %d (fp8): the reference's own torch::matmul has no Float8 kernel; bf16, f16 and f32 experts are supported", cfg->dtype);
   if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16 && cfg->dtype != B2M_DTYPE_F32) return fail(nullptr, B2M_EINVAL, "bad dtype");
@@ -790,7 +792,10 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
     make_fp8_shape(&shape);
   }
   if (int4) {
-    if (cfg->dtype != B2M_DTYPE_BF16)
+    if (int4_f16 && cfg->dtype != B2M_DTYPE_F16)
+      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights with fp16 scales need an f16 model dtype (activations), got dtype %d",
+                  cfg->dtype);
+    if (!int4_f16 && cfg->dtype != B2M_DTYPE_BF16)
       return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights need a bf16 model dtype (activations), got dtype %d", cfg->dtype);
     if (cfg->expert_type != B2M_EXPERT_MIXTRAL_MOE_DENSE_ACT_DENSE && cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
       return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights support Mixtral (4) and DeepSeek (5) experts, got expert_type %d", cfg->expert_type);

@@ -95,7 +95,7 @@ struct GemmParams {
   const uint8_t* f8_s0;
   const uint8_t* f8_s1;
   size_t f8_slot_bytes;
-  // ---- int4 weights (int4_weights.cuh; bf16 activations): non-null = the A maps are uint8 maps over 4-bit code matrices and
+  // ---- int4 weights (int4_weights.cuh; bf16 or f16 activations): non-null = the A maps are uint8 maps over 4-bit code matrices and
   // i4_g0 / i4_g1 are the tile-major group grids (one uint32 per row and 128 k) of A0 / A1 in slot 0, i4_slot_bytes apart
   const uint8_t* i4_g0;
   const uint8_t* i4_g1;

@@ -134,9 +134,10 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
 // FP8 (AS_FP8: bf16, MC == 1, no m_rows / expert-parallel regions; every tile width): the A maps are uint8 maps over e4m3
 // matrices; the producer loads 8-KiB e4m3 tiles and the consumers dequantise their fragments with the tile's block scale
 // (fp8_weights.cuh) into the same register-A wgmmas, over the same tile walk and launch plan as the bf16 engine.
-// INT4 (AS_INT4: same restrictions and plan as FP8): the A maps are uint8 maps over the 4-bit code matrices (32-byte rows);
-// the producer loads 4-KiB code tiles and the consumers dequantise their fragments with the group words of their rows
-// (int4_weights.cuh), read from the tile-major group grids one k-block ahead.
+// INT4 (AS_INT4: same restrictions and plan as FP8, but bf16 or f16 -- the group scales are of the activations' type): the A
+// maps are uint8 maps over the 4-bit code matrices (32-byte rows); the producer loads 4-KiB code tiles and the consumers
+// dequantise their fragments with the group words of their rows (int4_weights.cuh), read from the tile-major group grids
+// one k-block ahead.
 template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, int AS = AS_BF16>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
                                           const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
@@ -155,7 +156,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
   int* pkf = cnts + MAX_E;             // PK: pk_ok of each expert's slot
   static_assert(!PK || (MC == 1 && DT == DT_BF16 && NT <= 64), "packed weights: bf16 decode-sized tiles");
   static_assert(!F8 || (MC == 1 && DT == DT_BF16), "fp8 weights: bf16 activations, single-CTA tiles");
-  static_assert(!I4 || (MC == 1 && DT == DT_BF16), "int4 weights: bf16 activations, single-CTA tiles");
+  static_assert(!I4 || (MC == 1 && (DT == DT_BF16 || DT == DT_F16)), "int4 weights: 16-bit activations, single-CTA tiles");
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -452,8 +453,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
           f8::decode_lane(sa, ct, s0, fa0[bf]);
           if constexpr (DUAL) f8::decode_lane(sa + A_BYTES, ct, s1, fa1[bf]);
         } else if constexpr (I4) {
-          i4::decode_lane(sa, ct, grp.cur[0][0], grp.cur[0][1], fa0[bf]);
-          if constexpr (DUAL) i4::decode_lane(sa + A_BYTES, ct, grp.cur[1][0], grp.cur[1][1], fa1[bf]);
+          i4::decode_lane<typename Half16<DT>::T>(sa, ct, grp.cur[0][0], grp.cur[0][1], fa0[bf]);
+          if constexpr (DUAL) i4::decode_lane<typename Half16<DT>::T>(sa + A_BYTES, ct, grp.cur[1][0], grp.cur[1][1], fa1[bf]);
         } else {
           wp::decode_lane(sa, ct, fa0[bf]);
           if constexpr (DUAL) wp::decode_lane(sa + A_BYTES, ct, fa1[bf]);
@@ -466,9 +467,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
           const uint64_t koff = (uint64_t)((k * MMA_K * 2) >> 4);
           const uint32_t acc = (kb != t.kb_begin || k > 0) ? 1u : 0u;
-          wgmma_rs_bf16<NT>(acc0, fa0[bf][4 * k], fa0[bf][4 * k + 1], fa0[bf][4 * k + 2], fa0[bf][4 * k + 3], db + koff, acc);
+          wgmma_rs<NT, DT>(acc0, fa0[bf][4 * k], fa0[bf][4 * k + 1], fa0[bf][4 * k + 2], fa0[bf][4 * k + 3], db + koff, acc);
           if constexpr (DUAL)
-            wgmma_rs_bf16<NT>(acc1, fa1[bf][4 * k], fa1[bf][4 * k + 1], fa1[bf][4 * k + 2], fa1[bf][4 * k + 3], db + koff, acc);
+            wgmma_rs<NT, DT>(acc1, fa1[bf][4 * k], fa1[bf][4 * k + 1], fa1[bf][4 * k + 2], fa1[bf][4 * k + 3], db + koff, acc);
         }
         next_stage();
       };
@@ -765,24 +766,23 @@ cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& g, const CUte
 template <int DT>
 static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
                                const GemmParams& p, int grid, cudaStream_t st) {
-  // int4 weights: every tile width the bf16 plan picks, same plan (the caller's p)
-  if constexpr (DT == DT_BF16) {
-    if (p.i4_g0) {
+  // int4 weights (bf16 or f16 scales and activations): every tile width the plan of the DT engine picks, same plan (the
+  // caller's p)
+  if (p.i4_g0) {
 #define B2M_ICASE(N)                                                                \
   case N:                                                                           \
     return dual ? launch_tc<N, true, DT, 1, AS_INT4>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
-      switch (nt) {
-        B2M_ICASE(16)
-        B2M_ICASE(32)
-        B2M_ICASE(64)
-        B2M_ICASE(128)
-        case 256:
-          return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
-        default:
-          return cudaErrorInvalidValue;
-      }
-#undef B2M_ICASE
+    switch (nt) {
+      B2M_ICASE(16)
+      B2M_ICASE(32)
+      B2M_ICASE(64)
+      B2M_ICASE(128)
+      case 256:
+        return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
+      default:
+        return cudaErrorInvalidValue;
     }
+#undef B2M_ICASE
   }
   // fp8 weights: every tile width the bf16 plan picks, same plan (the caller's p)
   if constexpr (DT == DT_BF16) {
@@ -985,7 +985,7 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
     return launch_grouped_gemm_tc(dtype, nt, dual, a0, a1, b, q, grid, st);
   }
   if (dtype == DT_BF16) return dispatch_nt<DT_BF16>(nt, dual, a0, a1, b, p, grid, st);
-  if (dtype == DT_F16 && !p.f8_s0 && !p.i4_g0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);
+  if (dtype == DT_F16 && !p.f8_s0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);   // (fp8 weights: bf16 only)
   return cudaErrorInvalidValue;
 }
 

@@ -52,9 +52,10 @@ class MoEEngine:
                  pack_weights: bool = True, expert_dtype: Optional[torch.dtype] = None):
         """expert_dtype: None = the routed experts are stored in `dtype`; torch.float8_e4m3fn = FP8 E4M3 with one fp32 scale
         per 128x128 block (`fp8.py`; `dtype` stays the activation dtype and must be bf16; register_expert / load_expert then
-        take the three e4m3 matrices and their scale grids); torch.uint4 = 4-bit codes with a bf16 scale and a 4-bit zero
-        point per 128 inputs (`int4.py`; `dtype` must be bf16; register_expert / load_expert then take the three packed code
-        matrices with scales= and zeros=)."""
+        take the three e4m3 matrices and their scale grids); torch.uint4 = 4-bit codes with a 16-bit scale and a 4-bit zero
+        point per 128 inputs (`int4.py`; register_expert / load_expert then take the three packed code matrices with scales=
+        and zeros=).  The scales are of `dtype`: bf16 (B2M_WEIGHTS_INT4_G128) or float16 (B2M_WEIGHTS_INT4_G128_F16, the
+        AWQ / GPTQ format: `int4.from_awq`, `int4.from_gptq`, `hf.load_int4_checkpoint`)."""
         self.lib = L.load()
         if not torch.cuda.is_available():
             raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -66,8 +67,8 @@ class MoEEngine:
         self.int4 = expert_dtype == torch.uint4
         if self.fp8 and dtype != torch.bfloat16:
             raise ValueError("fp8 experts compute with bf16 activations: dtype must be torch.bfloat16")
-        if self.int4 and dtype != torch.bfloat16:
-            raise ValueError("int4 experts compute with bf16 activations: dtype must be torch.bfloat16")
+        if self.int4 and dtype not in (torch.bfloat16, torch.float16):
+            raise ValueError("int4 experts compute with 16-bit activations: dtype must be torch.bfloat16 or torch.float16")
         self.dtype = dtype
         self.device = torch.device("cuda", device)
         self.L, self.E, self.H, self.I, self.k = num_layers, num_experts, hidden, inter, top_k
@@ -99,7 +100,11 @@ class MoEEngine:
         self.max_tokens = max_tokens
         h = C.c_void_p()
         torch.cuda.set_device(self.device)
-        fmt = L.WEIGHTS_FP8_E4M3_B128 if self.fp8 else L.WEIGHTS_INT4_G128 if self.int4 else L.WEIGHTS_MODEL_DTYPE
+        fmt = L.WEIGHTS_MODEL_DTYPE
+        if self.fp8:
+            fmt = L.WEIGHTS_FP8_E4M3_B128
+        elif self.int4:
+            fmt = L.WEIGHTS_INT4_G128_F16 if dtype == torch.float16 else L.WEIGHTS_INT4_G128
         L.check(None, self.lib.b2m_ctx_create_ex(C.byref(cfg), fmt, C.byref(h)))
         self._h = h
         self._blobs: Dict[Tuple[int, int], torch.Tensor] = {}
@@ -184,8 +189,8 @@ class MoEEngine:
             if t.dtype != torch.uint8 or tuple(t.shape) != (r, c // 2):
                 raise ValueError(f"expected a uint8 {(r, c // 2)} code matrix (two codes per byte), got {t.dtype} {tuple(t.shape)}")
             want = (r, c // I4.GROUP)
-            if s.dtype != torch.bfloat16 or tuple(s.shape) != want:
-                raise ValueError(f"expected a bfloat16 {want} scale grid, got {s.dtype} {tuple(s.shape)}")
+            if s.dtype != self.dtype or tuple(s.shape) != want:   # (the scales are of the activations' type: no rounding)
+                raise ValueError(f"expected a {self.dtype} {want} scale grid, got {s.dtype} {tuple(s.shape)}")
             if z.dtype != torch.uint8 or tuple(z.shape) != want:
                 raise ValueError(f"expected a uint8 {want} zero-point grid, got {z.dtype} {tuple(z.shape)}")
             parts.append(t.detach().contiguous().reshape(-1))
@@ -209,8 +214,8 @@ class MoEEngine:
         """Host-backed expert (can be staged in and evicted).  tensors: Mixtral (w1,w2,w3),
         DeepSeek (gate,up,down), Switch (wi,wo), NLLB/FSGPT (fc1,fc1_bias,fc2,fc2_bias) -- nn.Linear [out,in] layout.
         fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids.
-        int4 engine: the three uint8 [out, in/2] code matrices (int4.quantize_g128), `scales` (bfloat16 [out, in/128]) and
-        `zeros` (uint8 [out, in/128])."""
+        int4 engine: the three uint8 [out, in/2] code matrices (int4.quantize_g128), `scales` ([out, in/128] of the engine's
+        dtype, bfloat16 or float16) and `zeros` (uint8 [out, in/128])."""
         parts = self._quant_parts(tensors, scales, zeros)
         if parts is not None:
             blob = torch.zeros(self.expert_bytes, dtype=torch.uint8, pin_memory=pin)
@@ -252,7 +257,8 @@ class MoEEngine:
         issued (on the current stream) before the next forward of this layer; the second eager forward after the load packs
         the slot for the decode GEMMs (pack_weights=True); to change the weights later, call load_expert again and write through the view it returns.
         fp8 engine: `tensors` are the three float8_e4m3fn matrices and `scales` their float32 grids; the view is uint8.
-        int4 engine: `tensors` are the three uint8 code matrices, `scales` / `zeros` their bf16 / uint8 grids; the view is uint8."""
+        int4 engine: `tensors` are the three uint8 code matrices, `scales` / `zeros` their grids (the engine's dtype / uint8);
+        the view is uint8."""
         parts = None
         if tensors is not None:
             parts = self._quant_parts(tensors, scales, zeros)

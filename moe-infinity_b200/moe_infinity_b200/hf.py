@@ -1,5 +1,6 @@
 """HuggingFace plug-in helpers: run a `transformers` Mixtral or DeepSeek-V3 model with its MoE blocks executed by the CUDA
-engine (`patch_mixtral`, `patch_deepseek_v3`).
+engine (`patch_mixtral`, `patch_deepseek_v3`), and load the routed experts of a published AWQ / GPTQ 4-bit checkpoint into
+an f16 int4 engine as they are stored (`load_int4_checkpoint`).
 
 The reference achieves this by monkey-patching HF classes at load time (moe_infinity/runtime/model_offload.py:285-321:
 `MixtralSparseMoeBlock -> SyncMixtralSparseMoeBlock`).  The installed transformers (5.x) stores the experts of a layer as
@@ -9,7 +10,8 @@ PyTorch (same logits as HF) and hands everything after it to `MoEEngine.forward`
 """
 from __future__ import annotations
 
-from typing import Optional
+import contextlib
+from typing import Dict, List, Optional, Sequence, Union
 
 import torch
 import torch.nn as nn
@@ -23,13 +25,13 @@ from .engine import MoEEngine
 
 def _load(engine: MoEEngine, layer: int, expert: int, ws, resident: bool):
     """Hand one expert's bf16 matrices to `engine`, quantised first when the engine stores fp8 (`fp8.quantize_block128`) or
-    int4 (`int4.quantize_g128`) experts."""
+    int4 (`int4.quantize_g128`, with scales of the engine's dtype) experts."""
     kw = {}
     if engine.fp8:
         ws, scales = zip(*[F8.quantize_block128(w) for w in ws])
         kw = dict(scales=scales)
     elif engine.int4:
-        ws, scales, zeros = zip(*[I4.quantize_g128(w) for w in ws])
+        ws, scales, zeros = zip(*[I4.quantize_g128(w, scale_dtype=engine.dtype) for w in ws])
         kw = dict(scales=scales, zeros=zeros)
     if resident:
         engine.load_expert(layer, expert, ws, **kw)
@@ -131,3 +133,106 @@ def patch_deepseek_v3(model, max_tokens: int = 4096, num_slots: int = 0, device_
         engine.set_gate_bias(l, moe.gate.e_score_correction_bias.data)
         layers[l].mlp = B200DeepseekV3MoeAdapter(engine, l)
     return engine
+
+
+# ---------------------------------------------------------------- published AWQ / GPTQ checkpoints
+def _int4_method(qc: dict) -> str:
+    """Validate a checkpoint's `quantization_config` and return "awq", "gptq" or "gptq_v2"."""
+    method = str(qc.get("quant_method", "")).lower()
+    bits = qc.get("bits", qc.get("w_bit"))
+    group = qc.get("group_size", qc.get("q_group_size"))
+    if method not in ("awq", "gptq"):
+        raise ValueError(f"quant_method {method!r}: only 'awq' and 'gptq' 4-bit checkpoints are supported")
+    if bits != 4:
+        raise ValueError(f"{method} checkpoint with bits={bits}: only 4-bit weights are supported")
+    if group != I4.GROUP:
+        raise ValueError(f"{method} checkpoint with group_size={group}: only group size {I4.GROUP} is supported")
+    if method == "awq":
+        if not qc.get("zero_point", True):
+            raise ValueError("AWQ checkpoint with zero_point=false: only asymmetric (zero-point) AWQ is supported")
+        version = str(qc.get("version", "gemm")).lower()
+        if version != "gemm":
+            raise ValueError(f"AWQ checkpoint version {version!r}: only the 'gemm' packing is supported")
+        return "awq"
+    fmt = str(qc.get("checkpoint_format", "gptq")).lower()
+    if fmt not in ("gptq", "gptq_v2"):
+        raise ValueError(f"GPTQ checkpoint_format {fmt!r}: only 'gptq' and 'gptq_v2' are supported")
+    return fmt
+
+
+def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], quantization_config: dict, model_type: str,
+                         resident: bool = True) -> List[int]:
+    """Load the routed experts and router weights of a published AWQ or GPTQ 4-bit checkpoint (its safetensors `shards`,
+    its config's `quantization_config`, `model_type` "mixtral" or "deepseek_v2" / "deepseek_v3") into `engine`, an int4
+    engine with float16 activations (`MoEEngine(dtype=torch.float16, expert_dtype=torch.uint4)`), without changing a
+    weight (`int4.from_awq` / `int4.from_gptq`).  Tensors are read one at a time with `safetensors.safe_open`.
+
+    Mixtral: model.layers.{l}.block_sparse_moe.experts.{e}.w{1,2,3}.* and ...block_sparse_moe.gate.weight.  DeepSeek:
+    model.layers.{l}.mlp.experts.{e}.{gate,up,down}_proj.*, mlp.gate.weight (and mlp.gate.e_score_correction_bias for a V3
+    router) and mlp.shared_experts.*, whose dequantised weights are registered as the f16 shared expert; layers without
+    experts (no mlp.gate.weight) are skipped.  `resident=False` registers the experts as pinned host blobs (offload).
+    Refused with a message: bits other than 4, group sizes other than 128, AWQ without zero points or in a packing other
+    than "gemm", act-order GPTQ (a g_idx other than c // 128), and a missing tensor.  Returns the layers it loaded."""
+    from safetensors import safe_open
+
+    if not engine.int4 or engine.dtype != torch.float16:
+        raise ValueError("load_int4_checkpoint needs an int4 engine with float16 activations "
+                         "(MoEEngine(dtype=torch.float16, expert_dtype=torch.uint4))")
+    method = _int4_method(quantization_config)
+    mixtral = model_type == "mixtral"
+    if not mixtral and not model_type.startswith("deepseek"):
+        raise ValueError(f"model_type {model_type!r}: Mixtral and DeepSeek checkpoints are supported")
+    if mixtral != (engine.expert_type == L.EXPERT_MIXTRAL):
+        raise ValueError(f"model_type {model_type!r} does not match the engine's expert_type {engine.expert_type}")
+    if isinstance(shards, str):
+        shards = [shards]
+    parts = ("qweight", "qzeros", "scales")
+    with contextlib.ExitStack() as stack:
+        files = [stack.enter_context(safe_open(path, framework="pt", device="cpu")) for path in shards]
+        where: Dict[str, object] = {k: f for f in files for k in f.keys()}
+
+        def linear(prefix: str):
+            t = [where[f"{prefix}.{p}"].get_tensor(f"{prefix}.{p}") for p in parts]
+            if method == "awq":
+                return I4.from_awq(*t)
+            gi = f"{prefix}.g_idx"
+            g_idx = where[gi].get_tensor(gi) if gi in where else None
+            return I4.from_gptq(*t, g_idx=g_idx, checkpoint_format=method)
+
+        if mixtral:
+            layers = list(range(engine.L))
+            moe = "block_sparse_moe"
+            names = ("w1", "w2", "w3")                                 # reference order: w1 | w2 | w3
+        else:
+            layers = [l for l in range(engine.L) if f"model.layers.{l}.mlp.gate.weight" in where]
+            moe = "mlp"
+            names = ("gate_proj", "up_proj", "down_proj")              # DeepSeek order: gate | up | down
+        need = []
+        for l in layers:
+            base = f"model.layers.{l}.{moe}"
+            need.append(f"{base}.gate.weight")
+            need += [f"{base}.experts.{e}.{n}.{p}" for e in range(engine.E) for n in names for p in parts]
+            if not mixtral and engine.shared_inter > 0:
+                need += [f"{base}.shared_experts.{n}.{p}" for n in names for p in parts]
+            if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:
+                need.append(f"{base}.gate.e_score_correction_bias")
+        missing = [k for k in need if k not in where]
+        if missing:
+            raise ValueError(f"the checkpoint has no tensor {missing[0]} ({len(missing)} missing)")
+        for l in layers:
+            base = f"model.layers.{l}.{moe}"
+            for e in range(engine.E):
+                qs, ss, zs = zip(*[linear(f"{base}.experts.{e}.{n}") for n in names])
+                if resident:
+                    engine.load_expert(l, e, qs, scales=ss, zeros=zs)
+                else:
+                    engine.register_expert(l, e, qs, scales=ss, zeros=zs)
+            if not mixtral and engine.shared_inter > 0:
+                engine.register_shared(l, [I4.dequantize_g128(*linear(f"{base}.shared_experts.{n}"), torch.float16)
+                                           for n in names])
+            key = f"{base}.gate.weight"
+            engine.set_gate(l, where[key].get_tensor(key))
+            if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:
+                key = f"{base}.gate.e_score_correction_bias"
+                engine.set_gate_bias(l, where[key].get_tensor(key).float())
+    return layers

@@ -1,17 +1,20 @@
-"""4-bit integer expert weights with a bf16 scale and a 4-bit zero point per 128 inputs (W4A16 group quantisation).
+"""4-bit integer expert weights with a 16-bit scale and a 4-bit zero point per 128 inputs (W4A16 group quantisation).
 
-`MoEEngine(..., expert_dtype=torch.uint4)` runs such experts; the numbers it computes are defined by `dequantize_g128`: the
-bf16 engine on W = bf16(s[r][c // 128] * (q[r][c] - z[r][c // 128])), the exact product rounded once (include/b2m.h,
-B2M_WEIGHTS_INT4_G128).  `quantize_g128` turns a bf16 / fp32 checkpoint into that format; `pack_groups` builds the
-tile-major group grid an expert blob stores after its code matrices."""
+`MoEEngine(..., expert_dtype=torch.uint4)` runs such experts; the scales are of the engine's dtype T (bfloat16:
+B2M_WEIGHTS_INT4_G128; float16: B2M_WEIGHTS_INT4_G128_F16, the AWQ / GPTQ format).  The numbers it computes are defined by
+`dequantize_g128`: the T engine on W = T(s[r][c // 128] * (q[r][c] - z[r][c // 128])), the exact product rounded once
+(include/b2m.h).  `quantize_g128` turns a bf16 / fp32 checkpoint into that format; `from_awq` and `from_gptq` unpack the
+tensors of published AWQ / GPTQ checkpoints into it without changing a weight; `pack_groups` builds the tile-major group
+grid an expert blob stores after its code matrices."""
 from __future__ import annotations
 
-from typing import Tuple
+from typing import Optional, Tuple
 
 import torch
 
 GROUP = 128
 TILE_ROWS = 128   # rows of one GEMM tile: the group grid keeps a tile's 128 words of one group together
+SCALE_DTYPES = (torch.bfloat16, torch.float16)
 
 
 def _groups(rows: int, cols: int) -> int:
@@ -20,23 +23,28 @@ def _groups(rows: int, cols: int) -> int:
     return cols // GROUP
 
 
-def quantize_g128(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    """w [out, in] (any float dtype) -> (q uint8 [out, in / 2], s bfloat16 [out, in / 128], z uint8 [out, in / 128]).
+def quantize_g128(w: torch.Tensor, scale_dtype: torch.dtype = torch.bfloat16) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """w [out, in] (any float dtype) -> (q uint8 [out, in / 2], s scale_dtype [out, in / 128], z uint8 [out, in / 128]).
 
-    Asymmetric min/max round-to-nearest per group of 128 inputs of a row: s = bf16((max - min) / 15), rounded to bf16
-    BEFORE the codes are computed; z = clamp(round(-min / s), 0, 15); code = clamp(round(w / s) + z, 0, 15).  A group
-    whose scale rounds to zero (every all-equal group among them) gets s = bf16(max), z = 0 and every code 1, so it holds
-    bf16(max) exactly -- or s = 1, z = 0, codes 0 when bf16(max) is zero (an all-zero group).
+    Asymmetric min/max round-to-nearest per group of 128 inputs of a row: s = S((max - min) / 15) with S = scale_dtype
+    (bfloat16, or float16 for an f16 engine), rounded to S BEFORE the codes are computed; z = clamp(round(-min / s), 0, 15);
+    code = clamp(round(w / s) + z, 0, 15).  A group whose scale rounds to zero (every all-equal group among them) gets
+    s = S(max), z = 0 and every code 1, so it holds S(max) exactly -- or s = 1, z = 0, codes 0 when S(max) is zero (an
+    all-zero group).  A float16 scale that overflows is refused.
     q packs two codes per byte: column c in the low nibble of byte c // 2 when c is even, in the high nibble when odd."""
     if w.dim() != 2:
         raise ValueError("quantize_g128 takes a 2-D [out, in] matrix")
+    if scale_dtype not in SCALE_DTYPES:
+        raise ValueError(f"scale_dtype must be torch.bfloat16 or torch.float16, got {scale_dtype}")
     rows, cols = w.shape
     g = _groups(rows, cols)
     b = w.detach().float().reshape(rows, g, GROUP)
     mn, mx = b.amin(dim=2), b.amax(dim=2)
-    s = ((mx - mn) / 15).to(torch.bfloat16).float()
+    s = ((mx - mn) / 15).to(scale_dtype).float()
+    if scale_dtype == torch.float16 and not bool(torch.isfinite(s).all()):
+        raise ValueError("a group's range does not fit a float16 scale (max - min > 15 * 65504)")
     degenerate = s == 0
-    mxb = mx.to(torch.bfloat16).float()
+    mxb = mx.to(scale_dtype).float()
     s = torch.where(degenerate, torch.where(mxb == 0, torch.ones_like(s), mxb), s)
     z = torch.where(degenerate, torch.zeros_like(s), (-mn / s).round().clamp(0, 15))
     codes = ((b / s[..., None]).round() + z[..., None]).clamp(0, 15)
@@ -44,7 +52,7 @@ def quantize_g128(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Te
     codes = torch.where(degenerate[..., None], fill[..., None].expand_as(codes), codes)
     codes = codes.to(torch.uint8).reshape(rows, cols)
     q = codes[:, 0::2] | (codes[:, 1::2] << 4)
-    return q.contiguous(), s.to(torch.bfloat16).contiguous(), z.to(torch.uint8).contiguous()
+    return q.contiguous(), s.to(scale_dtype).contiguous(), z.to(torch.uint8).contiguous()
 
 
 def unpack_codes(q: torch.Tensor) -> torch.Tensor:
@@ -57,8 +65,8 @@ def _check(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> Tuple[int, int,
         raise ValueError(f"q must be a 2-D uint8 [out, in / 2] tensor, got {q.dtype} {tuple(q.shape)}")
     rows, cols = q.shape[0], 2 * q.shape[1]
     g = _groups(rows, cols)
-    if s.dtype != torch.bfloat16 or tuple(s.shape) != (rows, g):
-        raise ValueError(f"expected a bfloat16 {(rows, g)} scale grid, got {s.dtype} {tuple(s.shape)}")
+    if s.dtype not in SCALE_DTYPES or tuple(s.shape) != (rows, g):
+        raise ValueError(f"expected a bfloat16 or float16 {(rows, g)} scale grid, got {s.dtype} {tuple(s.shape)}")
     if z.dtype != torch.uint8 or tuple(z.shape) != (rows, g):
         raise ValueError(f"expected a uint8 {(rows, g)} zero-point grid, got {z.dtype} {tuple(z.shape)}")
     return rows, cols, g
@@ -66,7 +74,8 @@ def _check(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> Tuple[int, int,
 
 def dequantize_g128(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
     """The weights an int4 engine computes with: (s_expanded.float() * (q.float() - z_expanded.float())).to(dtype) -- an
-    exact fp32 product, one rounding.  Zero points above 15 are taken modulo 16, as the GEMMs read only 4 bits."""
+    exact fp32 product, one rounding (dtype = the engine's dtype, which is also the type of s; float16 products beyond
+    65504 become +-Inf).  Zero points above 15 are taken modulo 16, as the GEMMs read only 4 bits."""
     _check(q, s, z)
     codes = unpack_codes(q).float()
     se = s.float().repeat_interleave(GROUP, 1)
@@ -76,11 +85,11 @@ def dequantize_g128(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor, dtype: to
 
 def pack_groups(s: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
     """[out, in / 128] scales and zero points -> the matrix's group grid as it sits in an expert blob: one little-endian
-    uint32 (bf16 bits of s | z << 16) per (row, group), tile-major -- the word of (r, g) at index
+    uint32 (bf16 or fp16 bits of s | z << 16) per (row, group), tile-major -- the word of (r, g) at index
     ((r // 128) * (in / 128) + g) * 128 + r % 128.  Returned as a flat uint8 tensor."""
     rows, g = s.shape
-    if rows % TILE_ROWS or tuple(z.shape) != (rows, g) or s.dtype != torch.bfloat16 or z.dtype != torch.uint8:
-        raise ValueError("pack_groups takes bfloat16 scales and uint8 zero points of the same [out, in / 128] shape")
+    if rows % TILE_ROWS or tuple(z.shape) != (rows, g) or s.dtype not in SCALE_DTYPES or z.dtype != torch.uint8:
+        raise ValueError("pack_groups takes bfloat16 or float16 scales and uint8 zero points of the same [out, in / 128] shape")
     words = (s.view(torch.int16).to(torch.int32) & 0xffff) | ((z.to(torch.int32) & 15) << 16)
     words = words.reshape(rows // TILE_ROWS, TILE_ROWS, g).permute(0, 2, 1).contiguous()
     return words.view(torch.uint8).reshape(-1)
@@ -91,3 +100,83 @@ def expert_blob_bytes(hidden: int, inter: int) -> int:
     expert_blob_bytes)."""
     _groups(inter, hidden)
     return 3 * hidden * inter // 2 + 3 * (hidden * inter // GROUP) * 4
+
+
+# ---------------------------------------------------------------- published 4-bit checkpoints (AWQ, GPTQ)
+_AWQ_ORDER = (0, 2, 4, 6, 1, 3, 5, 7)   # nibble i of an AWQ word holds output row 8 j + _AWQ_ORDER[i]
+
+
+def _nibbles(w: torch.Tensor) -> torch.Tensor:
+    """int32 [..., n] -> its eight nibbles, least significant first: int64 [..., n, 8] in 0..15."""
+    return (w.to(torch.int64)[..., None] >> (4 * torch.arange(8, device=w.device))) & 15
+
+
+def _pack_codes(codes: torch.Tensor) -> torch.Tensor:
+    """[out, in] codes 0..15 -> [out, in / 2] bytes (column c in the low nibble of byte c // 2 when c is even)."""
+    codes = codes.to(torch.uint8)
+    return (codes[:, 0::2] | (codes[:, 1::2] << 4)).contiguous()
+
+
+def _checkpoint_groups(what: str, n_in: int, scales: torch.Tensor, n_out: int) -> int:
+    if scales.dtype != torch.float16 or scales.dim() != 2 or scales.shape[1] != n_out:
+        raise ValueError(f"{what} scales must be float16 [in / group, {n_out}], got {scales.dtype} {tuple(scales.shape)}")
+    if scales.shape[0] * GROUP != n_in:
+        raise ValueError(f"{what}: only group size {GROUP} is supported ({n_in} inputs, {scales.shape[0]} groups)")
+    return scales.shape[0]
+
+
+def _check_int32(name: str, t: torch.Tensor, shape: Tuple[int, int]):
+    if t.dtype != torch.int32 or tuple(t.shape) != shape:
+        raise ValueError(f"{name} must be int32 {shape}, got {t.dtype} {tuple(t.shape)}")
+
+
+def from_awq(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One AWQ ("gemm" version, zero_point=True, group size 128) linear layer -> (q, s, z) of this library: q uint8
+    [out, in / 2], s float16 [out, in / 128], z uint8 [out, in / 128].  No weight changes: `dequantize_g128(q, s, z,
+    torch.float16)` is AWQ's own (q - z) * s in fp16.
+
+    qweight int32 [in, out / 8]: nibble i of qweight[c, j] is the code of output row 8 j + (0, 2, 4, 6, 1, 3, 5, 7)[i];
+    qzeros int32 [in / 128, out / 8] in the same nibble order holds z; scales float16 [in / 128, out]."""
+    if qweight.dim() != 2:
+        raise ValueError(f"AWQ qweight must be int32 [in, out / 8], got {qweight.dtype} {tuple(qweight.shape)}")
+    n_in, n_out = qweight.shape[0], 8 * qweight.shape[1]
+    _check_int32("AWQ qweight", qweight, (n_in, n_out // 8))
+    g = _checkpoint_groups("AWQ", n_in, scales, n_out)
+    _check_int32("AWQ qzeros", qzeros, (g, n_out // 8))
+    _groups(n_out, n_in)
+    inv = [_AWQ_ORDER.index(p) for p in range(8)]                  # row 8 j + p sits in nibble inv[p]
+    codes = _nibbles(qweight)[..., inv].reshape(n_in, n_out).t()
+    z = _nibbles(qzeros)[..., inv].reshape(g, n_out).t()
+    return _pack_codes(codes), scales.t().contiguous(), z.to(torch.uint8).contiguous()
+
+
+def from_gptq(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor, g_idx: Optional[torch.Tensor] = None,
+              checkpoint_format: str = "gptq") -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One GPTQ (4 bits, group size 128, no act-order) linear layer -> (q, s, z) of this library (as `from_awq`).  No weight
+    changes: `dequantize_g128(q, s, z, torch.float16)` is GPTQ's own (q - z) * s in fp16.
+
+    qweight int32 [in / 8, out]: nibble i of qweight[j, r] is input column 8 j + i; qzeros int32 [in / 128, out / 8]: nibble i
+    of qzeros[g, j] belongs to row 8 j + i; scales float16 [in / 128, out].  checkpoint_format "gptq" (v1) stores z - 1, so a
+    stored 15 (z = 16) cannot be represented and is refused; "gptq_v2" stores z.  g_idx, if given, must be c // 128
+    (act-order checkpoints are refused)."""
+    if checkpoint_format not in ("gptq", "gptq_v2"):
+        raise ValueError(f"GPTQ checkpoint_format must be 'gptq' or 'gptq_v2', got {checkpoint_format!r}")
+    if qweight.dim() != 2:
+        raise ValueError(f"GPTQ qweight must be int32 [in / 8, out], got {qweight.dtype} {tuple(qweight.shape)}")
+    n_in, n_out = 8 * qweight.shape[0], qweight.shape[1]
+    _check_int32("GPTQ qweight", qweight, (n_in // 8, n_out))
+    g = _checkpoint_groups("GPTQ", n_in, scales, n_out)
+    _check_int32("GPTQ qzeros", qzeros, (g, n_out // 8))
+    _groups(n_out, n_in)
+    if g_idx is not None:
+        want = torch.arange(n_in, device=g_idx.device) // GROUP
+        if tuple(g_idx.shape) != (n_in,) or not torch.equal(g_idx.to(torch.int64), want):
+            raise ValueError("GPTQ g_idx is not c // 128: act-order (desc_act) checkpoints are not supported")
+    codes = _nibbles(qweight).permute(0, 2, 1).reshape(n_in, n_out).t()
+    z = _nibbles(qzeros).reshape(g, n_out).t()
+    if checkpoint_format == "gptq":
+        if bool((z == 15).any()):
+            raise ValueError("GPTQ qzeros holds 15, i.e. a zero point of 16 in the v1 format (stored z - 1), "
+                             "which 4 bits cannot represent")
+        z = z + 1
+    return _pack_codes(codes), scales.t().contiguous(), z.to(torch.uint8).contiguous()
