@@ -222,6 +222,16 @@ int b2m_ctx_destroy(b2m_ctx* ctx);
                                        points return B2M_EUNSUPPORTED on such a context. */
 /* b2m_ctx_create with the routed experts stored in `weight_format` (B2M_WEIGHTS_*; any other value: B2M_EINVAL) */
 int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out);
+/* B2M_WEIGHTS_INT4_G128_F16 only: act-order GPTQ (desc_act).  `dev_perm` is a borrowed device table uint16 [E][H] (like the
+ * gate weight): column j of every row the routing kernels gather for expert e is x[t][dev_perm[e * H + j]], so expert e's
+ * gate/up matrices are stored with their input columns in that order (W[:, P], whose 128-column groups are then contiguous;
+ * the down projection's permutation is applied to the stored matrices at load time and needs no table).  NULL returns the
+ * layer to natural order.  The table is read by every routing call of the layer (b2m_moe_forward, b2m_route,
+ * b2m_route_from_mask); a captured graph keeps the pointer it was captured with and reads the table's contents at replay.
+ * B2M_WS_XP and B2M_WS_HMID rows of such a layer hold permuted activations.  An entry >= H reads as 0 and sets a bit of the
+ * sticky device error word (B2M_EINVAL from b2m_check_errors / b2m_expert_outputs); nothing faults.  B2M_EUNSUPPORTED on a
+ * context of any other weight format, B2M_EINVAL for a layer out of range. */
+int b2m_set_input_perm(b2m_ctx* ctx, int layer, const uint16_t* dev_perm);
 
 /* replaces: prefetch_handle.offload/register + set_topology for an expert stage + expert_dispatcher.register_expert
  * (core/parallel/expert_dispatcher.cpp:160-173; blob layout core/model/model_topology.cpp:429-431:
@@ -278,7 +288,8 @@ int b2m_combine(b2m_ctx* ctx, int layer, const void* x, int T, void* out, void* 
  * ascending expert id, ascending token order inside an expert; `offsets_host` (E+1 ints) may be NULL */
 int b2m_expert_outputs(b2m_ctx* ctx, int T, void* out_rows, int* offsets_host, void* stream);
 /* synchronises `stream` and reports (then clears) the sticky device error word; B2M_EINVAL when a mask handed to
- * b2m_route_from_mask had a row with more than top_k experts (the reference would run them all: expert_dispatcher.cpp:274-285) */
+ * b2m_route_from_mask had a row with more than top_k experts (the reference would run them all: expert_dispatcher.cpp:274-285),
+ * or when a table set with b2m_set_input_perm held an entry >= H */
 int b2m_check_errors(b2m_ctx* ctx, void* stream);
 
 /* workspace access for tests / EP plumbing (device pointers owned by the context) */

@@ -141,6 +141,7 @@ struct b2m_ctx {
   int stage_pos = 0;
   std::vector<const void*> gate_w;  // per layer device pointers
   std::vector<const float*> gate_bias;  // B2M_ROUTER_DEEPSEEK_V3: per layer e_score_correction_bias [E] (device, borrowed)
+  std::vector<const uint16_t*> input_perm;  // B2M_WEIGHTS_INT4_G128_F16: per layer [E][H] gather table (device, borrowed) or null
 
   // workspace
   int cap_T = 0, cap_R = 0;
@@ -724,6 +725,7 @@ RouteParams base_route_params(b2m_ctx* c, int layer, const void* x, int T, int s
   p.xp = c->d_xp;
   p.ticket = c->d_ticket;
   p.err_flag = c->d_err;
+  p.input_perm = c->input_perm[layer];
   return p;
 }
 
@@ -904,6 +906,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   c->row_dirty.assign(L, 1);
   c->gate_w.assign(L, nullptr);
   c->gate_bias.assign(L, nullptr);
+  c->input_perm.assign(L, nullptr);
   CKC(cudaMalloc((void**)&c->d_slot_of, sizeof(int) * L * E));
   CKC(cudaMemset(c->d_slot_of, 0xff, sizeof(int) * L * E));
   CKC(cudaHostAlloc((void**)&c->h_stage, sizeof(int) * STAGE_RING * E, cudaHostAllocDefault));
@@ -1071,6 +1074,16 @@ int b2m_set_gate_bias(b2m_ctx* c, int layer, const float* dev_bias) {
                 B2M_ROUTER_DEEPSEEK_V3, c->cfg.router);
   if (!dev_bias) return fail(c, B2M_EINVAL, "b2m_set_gate_bias: dev_bias is null");
   c->gate_bias[layer] = dev_bias;
+  return B2M_OK;
+}
+
+int b2m_set_input_perm(b2m_ctx* c, int layer, const uint16_t* dev_perm) {
+  int r = check_layer(c, layer);
+  if (r) return r;
+  if (!c->int4 || c->cfg.dtype != B2M_DTYPE_F16)
+    return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations (act-order GPTQ) need a B2M_WEIGHTS_INT4_G128_F16 "
+                "context");
+  c->input_perm[layer] = dev_perm;
   return B2M_OK;
 }
 
@@ -1682,6 +1695,14 @@ int b2m_moe_forward(b2m_ctx* c, int layer, const void* x, const void* router_in,
   return b2m_combine(c, layer, x, T, out, stream);
 }
 
+// B2M_EINVAL naming what each bit of the (already cleared) sticky device error word reports
+static int fail_err_word(b2m_ctx* c, int bits) {
+  std::string what;
+  if (bits & 1) what += "a router-mask row names more experts than top_k (rows would be dropped)";
+  if (bits & 2) what += std::string(what.empty() ? "" : "; ") + "an input-permutation entry (b2m_set_input_perm) is >= hidden (read as 0)";
+  return fail(c, B2M_EINVAL, "device error word %d: %s", bits, what.c_str());
+}
+
 int b2m_expert_outputs(b2m_ctx* c, int T, void* out_rows, int* offsets_host, void* stream) {
   if (!c) return B2M_EINVAL;
   if (T < 0 || T > c->cap_T) return fail(c, B2M_EINVAL, "T=%d exceeds workspace capacity %d", T, c->cap_T);
@@ -1699,7 +1720,7 @@ int b2m_expert_outputs(b2m_ctx* c, int T, void* out_rows, int* offsets_host, voi
     if (*c->h_err) {
       const int bits = *c->h_err;
       CK(c, cudaMemsetAsync(c->d_err, 0, sizeof(int), st));
-      return fail(c, B2M_EINVAL, "device error word %d: a router-mask row names more experts than top_k=%d (rows would be dropped)", bits, c->cfg.top_k);
+      return fail_err_word(c, bits);
     }
   }
   return B2M_OK;
@@ -1713,7 +1734,7 @@ int b2m_check_errors(b2m_ctx* c, void* stream) {
   if (*c->h_err) {
     const int bits = *c->h_err;
     CK(c, cudaMemsetAsync(c->d_err, 0, sizeof(int), st));
-    return fail(c, B2M_EINVAL, "device error word %d: a router-mask row names more experts than top_k=%d", bits, c->cfg.top_k);
+return fail_err_word(c, bits);
   }
   return B2M_OK;
 }

@@ -197,7 +197,10 @@ struct RouteParams {
   float* y_zero;             // optional fp32 buffer to clear (split-K accumulator), y_zero_elems floats
   size_t y_zero_elems;
   int* ticket;               // small-T path: CTA arrival counter (0 between launches)
-  int* err_flag;             // sticky device error word (bit0: a mask row had more than k experts)
+  int* err_flag;             // sticky device error word (bit0: a mask row had more than k experts, bit1: an input-permutation
+                             // entry >= H)
+  const uint16_t* input_perm;  // null, or the layer's [E][H] table (b2m_set_input_perm): column c of a gathered row of expert e
+                               // is x[t][input_perm[e * H + c]]
   int rows_by_gate;          // with offsets_early: the last gate/top-k CTA also publishes row_of / perm_token, and the permute
                              // kernel only copies rows (no redundant ranking in each of its CTAs)
   int offsets_early;         // small-T path: the last gate/top-k CTA already publishes counts/offsets (so the gate/up GEMM can

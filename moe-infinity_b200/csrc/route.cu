@@ -597,24 +597,64 @@ __device__ __forceinline__ void chunk_rank_strided(const RouteParams& p, int t0,
   }
 }
 
-// Copy gathered rows x[t] -> xp[row] with 16-byte vectors; `nrows` (token,slot) pairs starting at token t0.
-__device__ void copy_rows_block(const RouteParams& p, int t0, int npairs, const int* s_rows, int warp0, int nwarps) {
-  const int lane = threadIdx.x & 31;
-  const int warp = (threadIdx.x >> 5) - warp0;
+// Gather of one 16-bit row through an input permutation (b2m_set_input_perm): dst[c] = src[perm[c]], 8 table entries per
+// 16-byte load, 8 independent 2-byte loads of the source row (L1-resident after the first touch), one 16-byte store; threads
+// tid, tid + nthr, ... of the caller share the row.  An entry >= H reads as 0 and sets bit 1 of the sticky error word
+// (b2m_check_errors); nothing outside src is read.  Not inlined: the routing kernels are instruction-cache cold every
+// launch, and layers without a table should not fetch this code (scalar arguments: no RouteParams copy for the call).
+__device__ __noinline__ void gather_row_perm(const uint16_t* __restrict__ src, const uint16_t* __restrict__ perm,
+                                             uint4* __restrict__ dst, int H, int tid, int nthr, int* err_flag) {
+  bool bad = false;
+  for (int v = tid; v < H / 8; v += nthr) {
+    const uint4 iv = reinterpret_cast<const uint4*>(perm)[v];
+    const uint16_t* ix = reinterpret_cast<const uint16_t*>(&iv);
+    uint4 o;
+    uint16_t* os = reinterpret_cast<uint16_t*>(&o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const bool ok = ix[j] < H;
+      bad |= !ok;
+      os[j] = ok ? src[ix[j]] : (uint16_t)0;
+    }
+    dst[v] = o;
+  }
+  if (bad && err_flag) atomicOr(err_flag, 2);
+}
+
+// Copy one activation row x[t] -> dst with 16-byte vectors, NTHR threads (a warp or the whole CTA; `tid` = this thread's
+// index among them).  e = the expert of the row: a layer with an input permutation gathers column c from x[t][perm[e][c]]
+// instead (gather_row_perm; 16-bit models only).
+template <int NTHR>
+__device__ __forceinline__ void copy_row(const RouteParams& p, int t, int e, void* dst_row, int tid) {
   const size_t rb = row_bytes(p);
   const int vec_per_row = (int)(rb / 16);   // uint4 = 8 x 16-bit (4 x fp32)
-  for (int i = warp; i < npairs; i += nwarps) {
-    const int row = s_rows[i];
-    const int t = t0 + i / p.k;
-    if (row < 0 || t >= p.T) continue;
-    const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + (size_t)t * rb);
-    uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb);
-    int v = lane;
+  const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + (size_t)t * rb);
+  uint4* dst = reinterpret_cast<uint4*>(dst_row);
+  if (p.input_perm) {
+    gather_row_perm(reinterpret_cast<const uint16_t*>(src), p.input_perm + (size_t)e * p.H, dst, p.H, tid, NTHR, p.err_flag);
+    return;
+  }
+  int v = tid;
+  if (NTHR == 32) {
     for (; v + 96 < vec_per_row; v += 128) {   // 4 independent 16 B loads in flight per lane
       const uint4 a = src[v], b = src[v + 32], c = src[v + 64], d = src[v + 96];
       dst[v] = a; dst[v + 32] = b; dst[v + 64] = c; dst[v + 96] = d;
     }
-    for (; v < vec_per_row; v += 32) dst[v] = src[v];
+  }
+  for (; v < vec_per_row; v += NTHR) dst[v] = src[v];
+}
+
+// Copy gathered rows x[t] -> xp[row], one warp per row; `npairs` (token,slot) pairs starting at token t0.
+__device__ void copy_rows_block(const RouteParams& p, int t0, int npairs, const int* s_rows, int warp0, int nwarps) {
+  const int lane = threadIdx.x & 31;
+  const int warp = (threadIdx.x >> 5) - warp0;
+  const size_t rb = row_bytes(p);
+  for (int i = warp; i < npairs; i += nwarps) {
+    const int row = s_rows[i];
+    const int t = t0 + i / p.k;
+    if (row < 0 || t >= p.T) continue;
+    const int e = p.input_perm ? p.topk_idx[(size_t)t0 * p.k + i] : 0;
+    copy_row<32>(p, t, e, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, lane);
   }
 }
 
@@ -930,13 +970,11 @@ __global__ void __launch_bounds__(RT_THREADS) permute_small_kernel(const RoutePa
   if (p.rows_by_gate) {
     // the gate/top-k kernel already published counts, offsets and the row maps: this kernel is a pure row copy
     const size_t rb = row_bytes(p);
-    const int vpr = (int)(rb / 16);
     for (int i = blockIdx.x; i < npairs; i += gridDim.x) {
       const int row = p.row_of[i];
       if (row < 0) continue;
-      const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + (size_t)(i / p.k) * rb);
-      uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb);
-      for (int v = threadIdx.x; v < vpr; v += RT_THREADS) dst[v] = src[v];
+      const int e = p.input_perm ? p.topk_idx[i] : 0;
+      copy_row<RT_THREADS>(p, i / p.k, e, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, threadIdx.x);
     }
     if (p.y_zero) {
       float4* z = reinterpret_cast<float4*>(p.y_zero);
@@ -1030,23 +1068,21 @@ __global__ void __launch_bounds__(RT_THREADS) permute_small_kernel(const RoutePa
   __syncthreads();
   // gather: CTA b copies rows b, b+grid, ...; the whole CTA moves one row (H*2 bytes) with 16 B vectors
   const size_t rb = row_bytes(p);
-  const int vec_per_row = (int)(rb / 16);
   for (int i = blockIdx.x; i < npairs; i += gridDim.x) {
     const int row = s_rows[i];
     if (row < 0) continue;
     const int t = i / p.k;
-    const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + (size_t)t * rb);
-    uint4* dst;
+    void* dst;
     if (p.ep_dispatch) {
       // expert-parallel: the row goes to the rank that owns its expert (peer memory over NVLink, or the send buffer)
       const int El = p.E / p.ep.nranks;
       const int e = s_idx[i];
       const int r = e / El;
-      dst = reinterpret_cast<uint4*>(ep_send_row(p.ep, r, row - s_off[r * El]));
+      dst = ep_send_row(p.ep, r, row - s_off[r * El]);
     } else {
-      dst = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb);
+      dst = reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb;
     }
-    for (int v = threadIdx.x; v < vec_per_row; v += RT_THREADS) dst[v] = src[v];
+    copy_row<RT_THREADS>(p, t, s_idx[i], dst, threadIdx.x);
   }
   if (p.ep_dispatch && p.ep.p2p) p2p_signal(p.ep, 0);
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 3);

@@ -56,6 +56,7 @@ SYMBOLS = [
     ("b2m_register_shared", _I, [_VP, _I, _VP, _SZ]),
     ("b2m_set_gate", _I, [_VP, _I, _VP]),
     ("b2m_set_gate_bias", _I, [_VP, _I, _VP]),
+    ("b2m_set_input_perm", _I, [_VP, _I, _VP]),
     ("b2m_host_pin", _I, [_VP, _VP, _SZ]),
     ("b2m_host_unpin", _I, [_VP, _VP]),
     ("b2m_make_resident", _I, [_VP, _I, _I, _I, _VP]),

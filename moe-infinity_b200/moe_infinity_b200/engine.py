@@ -110,6 +110,7 @@ class MoEEngine:
         self._blobs: Dict[Tuple[int, int], torch.Tensor] = {}
         self._gates: Dict[int, torch.Tensor] = {}
         self._biases: Dict[int, torch.Tensor] = {}
+        self._perms: Dict[int, torch.Tensor] = {}
         es = self.esize = 4 if dtype == torch.float32 else 2   # fp32 experts (dtype int 1) run on the CUDA-core fp32 path
         if expert_type in (L.EXPERT_NLLB, L.EXPERT_FSGPT):     # fc1 | fc1_bias | fc2 | fc2_bias (expert_module.cpp:70-77)
             self.expert_bytes = 2 * hidden * inter * es + (inter + hidden) * es
@@ -301,6 +302,24 @@ class MoEEngine:
         b = bias.detach().to(self.device, torch.float32).contiguous()
         self._biases[layer] = b                # borrowed by the context: keep it alive
         self._ck(self.lib.b2m_set_gate_bias(self._h, layer, C.c_void_p(b.data_ptr())))
+
+    def set_input_perm(self, layer: int, perm: Optional[torch.Tensor]):
+        """Act-order GPTQ on an f16 int4 engine (B2M_WEIGHTS_INT4_G128_F16): perm int [E, H], row e a permutation of
+        0..H-1 (`int4.from_gptq_act_order`); the routing kernels gather column j of expert e's rows from x[t][perm[e][j]],
+        so expert e's gate/up matrices are loaded as W[:, perm[e]].  None returns the layer to natural order.  The
+        workspace rows "xp" and "hmid" of such a layer hold permuted activations."""
+        if perm is None:
+            self._ck(self.lib.b2m_set_input_perm(self._h, layer, None))
+            self._perms.pop(layer, None)
+            return
+        if perm.dtype not in (torch.int16, torch.int32, torch.int64, torch.uint16) or tuple(perm.shape) != (self.E, self.H):
+            raise ValueError(f"expected an integer [{self.E}, {self.H}] permutation table, got {perm.dtype} {tuple(perm.shape)}")
+        p = perm.detach().to(torch.int64)
+        if self.H > 65536 or not torch.equal(p.sort(dim=1).values.cpu(), torch.arange(self.H).expand(self.E, self.H)):
+            raise ValueError("every row of the input permutation must be a permutation of 0..H-1")
+        t = p.to(torch.int32).to(torch.uint16).to(self.device).contiguous()
+        self._ck(self.lib.b2m_set_input_perm(self._h, layer, C.c_void_p(t.data_ptr())))
+        self._perms[layer] = t                 # borrowed by the context: keep it alive
 
     # ------------------------------------------------------------------ hot path
     def _router_args(self, router_logits, scores):

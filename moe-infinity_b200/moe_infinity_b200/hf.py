@@ -161,7 +161,7 @@ def _int4_method(qc: dict) -> str:
 
 
 def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], quantization_config: dict, model_type: str,
-                         resident: bool = True) -> List[int]:
+                         resident: bool = True, act_order: bool = False) -> List[int]:
     """Load the routed experts and router weights of a published AWQ or GPTQ 4-bit checkpoint (its safetensors `shards`,
     its config's `quantization_config`, `model_type` "mixtral" or "deepseek_v2" / "deepseek_v3") into `engine`, an int4
     engine with float16 activations (`MoEEngine(dtype=torch.float16, expert_dtype=torch.uint4)`), without changing a
@@ -171,8 +171,14 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
     model.layers.{l}.mlp.experts.{e}.{gate,up,down}_proj.*, mlp.gate.weight (and mlp.gate.e_score_correction_bias for a V3
     router) and mlp.shared_experts.*, whose dequantised weights are registered as the f16 shared expert; layers without
     experts (no mlp.gate.weight) are skipped.  `resident=False` registers the experts as pinned host blobs (offload).
+    act_order=True loads act-order GPTQ (desc_act, a g_idx other than c // 128) as well, without changing a weight: per
+    expert, P = the gate/up order and P2 = the down projection's (`int4.from_gptq_act_order`); the engine stores
+    gate/up as W[P2][:, P] and down as W[:, P2] (so the gate/up GEMM writes h[P2], which the down projection consumes),
+    and each layer with a non-identity P gets one [E, H] gather table (`MoEEngine.set_input_perm`).  The gate and up
+    projections of an expert must share their g_idx (GPTQ derives both from the same input Hessian); a checkpoint where
+    they differ is refused, naming the layer and expert.
     Refused with a message: bits other than 4, group sizes other than 128, AWQ without zero points or in a packing other
-    than "gemm", act-order GPTQ (a g_idx other than c // 128), and a missing tensor.  Returns the layers it loaded."""
+    than "gemm", act-order GPTQ without act_order=True, and a missing tensor.  Returns the layers it loaded."""
     from safetensors import safe_open
 
     if not engine.int4 or engine.dtype != torch.float16:
@@ -192,12 +198,29 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
         where: Dict[str, object] = {k: f for f in files for k in f.keys()}
 
         def linear(prefix: str):
+            """(q, s, z, perm) of one linear layer: (q, s, z) hold W[:, perm]; perm is None for natural column order."""
             t = [where[f"{prefix}.{p}"].get_tensor(f"{prefix}.{p}") for p in parts]
             if method == "awq":
-                return I4.from_awq(*t)
+                return (*I4.from_awq(*t), None)
             gi = f"{prefix}.g_idx"
             g_idx = where[gi].get_tensor(gi) if gi in where else None
-            return I4.from_gptq(*t, g_idx=g_idx, checkpoint_format=method)
+            if act_order and g_idx is not None:
+                q, s_, z, perm = I4.from_gptq_act_order(*t, g_idx, checkpoint_format=method)
+                return q, s_, z, (None if torch.equal(perm, torch.arange(perm.numel())) else perm)
+            if g_idx is not None and not torch.equal(g_idx.to(torch.int64), torch.arange(g_idx.numel()) // I4.GROUP):
+                raise ValueError(f"{prefix}: GPTQ g_idx is not c // 128, an act-order (desc_act) checkpoint: "
+                                 "load it with act_order=True")
+            return (*I4.from_gptq(*t, g_idx=g_idx, checkpoint_format=method), None)
+
+        def shared(prefix: str) -> torch.Tensor:
+            """A shared expert's linear layer dequantised to f16 in its natural column order."""
+            q, s_, z, perm = linear(prefix)
+            w = I4.dequantize_g128(q, s_, z, torch.float16)
+            return w if perm is None else w[:, perm.argsort()]
+
+        def rows(qsz, perm):
+            """(q, s, z) with their rows permuted (each row keeps its own scale and zero words)."""
+            return tuple(t[perm].contiguous() for t in qsz) if perm is not None else qsz
 
         if mixtral:
             layers = list(range(engine.L))
@@ -219,17 +242,30 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
         missing = [k for k in need if k not in where]
         if missing:
             raise ValueError(f"the checkpoint has no tensor {missing[0]} ({len(missing)} missing)")
+        (g_, u_), d_ = ((0, 2), 1) if mixtral else ((0, 1), 2)   # positions of gate, up and down in `names`
         for l in layers:
             base = f"model.layers.{l}.{moe}"
+            table = torch.arange(engine.H).repeat(engine.E, 1)
             for e in range(engine.E):
-                qs, ss, zs = zip(*[linear(f"{base}.experts.{e}.{n}") for n in names])
+                mats = [linear(f"{base}.experts.{e}.{n}") for n in names]
+                pg, pu, p2 = mats[g_][3], mats[u_][3], mats[d_][3]
+                if not (pg is None and pu is None) and (pg is None or pu is None or not torch.equal(pg, pu)):
+                    raise ValueError(f"layer {l} expert {e}: {names[g_]} and {names[u_]} have different g_idx; act-order "
+                                     "experts must share one input order for both (one permutation of the routed rows)")
+                if pg is not None:
+                    table[e] = pg
+                qsz = [m[:3] for m in mats]
+                for i in (g_, u_):
+                    qsz[i] = rows(qsz[i], p2)            # gate/up rows in the down projection's input order
+                qs, ss, zs = zip(*qsz)
                 if resident:
                     engine.load_expert(l, e, qs, scales=ss, zeros=zs)
                 else:
                     engine.register_expert(l, e, qs, scales=ss, zeros=zs)
+            if act_order and not torch.equal(table, torch.arange(engine.H).expand(engine.E, engine.H)):
+                engine.set_input_perm(l, table)
             if not mixtral and engine.shared_inter > 0:
-                engine.register_shared(l, [I4.dequantize_g128(*linear(f"{base}.shared_experts.{n}"), torch.float16)
-                                           for n in names])
+                engine.register_shared(l, [shared(f"{base}.shared_experts.{n}") for n in names])
             key = f"{base}.gate.weight"
             engine.set_gate(l, where[key].get_tensor(key))
             if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:

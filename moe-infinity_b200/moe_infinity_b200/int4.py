@@ -4,8 +4,9 @@
 B2M_WEIGHTS_INT4_G128; float16: B2M_WEIGHTS_INT4_G128_F16, the AWQ / GPTQ format).  The numbers it computes are defined by
 `dequantize_g128`: the T engine on W = T(s[r][c // 128] * (q[r][c] - z[r][c // 128])), the exact product rounded once
 (include/b2m.h).  `quantize_g128` turns a bf16 / fp32 checkpoint into that format; `from_awq` and `from_gptq` unpack the
-tensors of published AWQ / GPTQ checkpoints into it without changing a weight; `pack_groups` builds the tile-major group
-grid an expert blob stores after its code matrices."""
+tensors of published AWQ / GPTQ checkpoints into it without changing a weight, and `from_gptq_act_order` unpacks an
+act-order GPTQ layer into it with its input columns permuted (`dequantize_g_idx` is GPTQ's own dequantisation of such a
+layer); `pack_groups` builds the tile-major group grid an expert blob stores after its code matrices."""
 from __future__ import annotations
 
 from typing import Optional, Tuple
@@ -159,6 +160,18 @@ def from_gptq(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor,
     of qzeros[g, j] belongs to row 8 j + i; scales float16 [in / 128, out].  checkpoint_format "gptq" (v1) stores z - 1, so a
     stored 15 (z = 16) cannot be represented and is refused; "gptq_v2" stores z.  g_idx, if given, must be c // 128
     (act-order checkpoints are refused)."""
+    n_in = 8 * qweight.shape[0] if qweight.dim() == 2 else 0
+    codes, s, z = _gptq_unpack(qweight, qzeros, scales, checkpoint_format)
+    if g_idx is not None:
+        want = torch.arange(n_in, device=g_idx.device) // GROUP
+        if tuple(g_idx.shape) != (n_in,) or not torch.equal(g_idx.to(torch.int64), want):
+            raise ValueError("GPTQ g_idx is not c // 128: act-order (desc_act) checkpoints are not supported")
+    return _pack_codes(codes), s, z
+
+
+def _gptq_unpack(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor,
+                 checkpoint_format: str) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """GPTQ tensors -> (codes int64 [out, in] in the checkpoint's column order, s float16 [out, groups], z uint8 [out, groups])."""
     if checkpoint_format not in ("gptq", "gptq_v2"):
         raise ValueError(f"GPTQ checkpoint_format must be 'gptq' or 'gptq_v2', got {checkpoint_format!r}")
     if qweight.dim() != 2:
@@ -168,10 +181,6 @@ def from_gptq(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor,
     g = _checkpoint_groups("GPTQ", n_in, scales, n_out)
     _check_int32("GPTQ qzeros", qzeros, (g, n_out // 8))
     _groups(n_out, n_in)
-    if g_idx is not None:
-        want = torch.arange(n_in, device=g_idx.device) // GROUP
-        if tuple(g_idx.shape) != (n_in,) or not torch.equal(g_idx.to(torch.int64), want):
-            raise ValueError("GPTQ g_idx is not c // 128: act-order (desc_act) checkpoints are not supported")
     codes = _nibbles(qweight).permute(0, 2, 1).reshape(n_in, n_out).t()
     z = _nibbles(qzeros).reshape(g, n_out).t()
     if checkpoint_format == "gptq":
@@ -179,4 +188,42 @@ def from_gptq(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor,
             raise ValueError("GPTQ qzeros holds 15, i.e. a zero point of 16 in the v1 format (stored z - 1), "
                              "which 4 bits cannot represent")
         z = z + 1
-    return _pack_codes(codes), scales.t().contiguous(), z.to(torch.uint8).contiguous()
+    return codes, scales.t().contiguous(), z.to(torch.uint8).contiguous()
+
+
+def act_order_perm(g_idx: torch.Tensor, n_in: int) -> torch.Tensor:
+    """An act-order GPTQ layer's g_idx [in] -> P = stable argsort(g_idx) (int64 [in]), the column order in which every
+    group is 128 consecutive columns: g_idx[P[j]] = j // 128.  Refused unless every group 0 .. in / 128 - 1 has exactly
+    128 columns (GPTQ with desc_act and group size 128 quantises 128 consecutive columns of its order per group)."""
+    if g_idx.dim() != 1 or g_idx.numel() != n_in or g_idx.dtype not in (torch.int32, torch.int64):
+        raise ValueError(f"GPTQ g_idx must be an int32 [{n_in}] vector, got {g_idx.dtype} {tuple(g_idx.shape)}")
+    gi = g_idx.to(torch.int64)
+    ng = n_in // GROUP
+    if bool((gi < 0).any()) or bool((gi >= ng).any()) or not bool((torch.bincount(gi, minlength=ng) == GROUP).all()):
+        raise ValueError(f"GPTQ g_idx does not put exactly {GROUP} columns in each of the {ng} groups")
+    return torch.sort(gi, stable=True).indices
+
+
+def from_gptq_act_order(qweight: torch.Tensor, qzeros: torch.Tensor, scales: torch.Tensor, g_idx: torch.Tensor,
+                        checkpoint_format: str = "gptq") -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One act-order GPTQ (desc_act=True, 4 bits, group size 128) linear layer W [out, in] -> (q, s, z, perm): (q, s, z)
+    of this library hold W[:, perm], whose groups are contiguous, and perm = `act_order_perm(g_idx)`.  No weight changes:
+    `dequantize_g128(q, s, z, torch.float16)[:, perm.argsort()]` is GPTQ's own dequantisation (`dequantize_g_idx`).
+    Since W x = W[:, perm] x[perm], an engine runs the layer on inputs gathered through perm (`MoEEngine.set_input_perm`).
+    Tensors as `from_gptq`; any g_idx with 128 columns per group is taken, c // 128 included (then perm is the identity)."""
+    codes, s, z = _gptq_unpack(qweight, qzeros, scales, checkpoint_format)
+    perm = act_order_perm(g_idx, codes.shape[1])
+    return _pack_codes(codes[:, perm]), s, z, perm
+
+
+def dequantize_g_idx(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor, g_idx: torch.Tensor,
+                     dtype: torch.dtype = torch.float16) -> torch.Tensor:
+    """GPTQ's own dequantisation of a layer in its checkpoint's column order: W[r][c] = dtype(s[r][g_idx[c]] * (q[r][c] -
+    z[r][g_idx[c]])), the exact product rounded once.  q uint8 [out, in / 2] (`unpack_codes` layout, natural columns), s
+    and z [out, in / 128] indexed by group; g_idx [in]."""
+    _, cols, ng = _check(q, s, z)
+    gi = g_idx.to(device=q.device, dtype=torch.int64)
+    if tuple(gi.shape) != (cols,) or bool((gi < 0).any()) or bool((gi >= ng).any()):
+        raise ValueError(f"g_idx must be [{cols}] group indices below {ng}")
+    codes = unpack_codes(q).float()
+    return (s.float()[:, gi] * (codes - (z & 15).float()[:, gi])).to(dtype)
