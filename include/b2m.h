@@ -74,6 +74,24 @@ extern "C" {
  * on a layer whose bias was never set returns B2M_ESTATE (whatever router_in_kind).  The combine is the DeepSeek one
  * (models/deepseek.py:115-137). */
 #define B2M_ROUTER_DEEPSEEK_V3 4
+/* Qwen2-MoE / Qwen3-MoE router (transformers Qwen2MoeTopKRouter, Qwen3MoeTopKRouter: identical).  Per token:
+ *   1. logits in the model dtype                           (F.linear in bf16/f16: the fp32 dot is rounded to the model dtype)
+ *   2. p = fp32 softmax of the logits
+ *   3. top_k experts by p                                  ties go to the lowest index
+ *   4. if norm_topk_prob: w /= (sum of the k weights, in selection order), for every k (k = 1 gives 1.0); no epsilon
+ *   5. the weights stay fp32 and are never scaled
+ * Accepted by b2m_ctx_create_ex (B2M_EINVAL with a message otherwise) only with expert_type
+ * B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE (gate|up|down, the HF tensor order), dtype bf16 or f16, n_group = topk_group = 1
+ * and routed_scaling_factor = 1.0; every weight format works with its own restrictions.  The router weight is an nn.Linear
+ * of the model, so gate_dtype is normally the model dtype; B2M_WS_LOGITS holds model-dtype logits, as for Mixtral.
+ * Combine (Qwen2MoeExperts + Qwen2MoeSparseMoeBlock), per element, experts in ascending id (index_add_ order):
+ *   acc = 0;  acc = round(acc + round(round(y) * w))       y: fp32 expert output, w: fp32 weight, round: to the model dtype
+ * shared_inter > 0 makes it a Qwen2-MoE layer with a GATED shared expert (b2m_set_shared_gate):
+ *   g = round(sigmoid(round(x . shared_expert_gate)))       (B2M_WS_SHARED_GATE; the sigmoid is PyTorch's CUDA formula)
+ *   out = round(acc + round(g * round(s)))                  s: fp32 shared-expert output (B2M_WS_Y_SHARED)
+ * With B2M_NUMERICS_FP32: acc += w * y, then acc += g * s, rounded once.  A forward or combine of a layer with shared experts
+ * and no gate returns B2M_ESTATE.  The expert-parallel entry points return B2M_EUNSUPPORTED on such a context. */
+#define B2M_ROUTER_QWEN_MOE 5
 
 /* numerics of epilogue + combine */
 #define B2M_NUMERICS_REFERENCE 0 /* replay the reference's per-ATen-op rounding to the model dtype */
@@ -248,6 +266,11 @@ int b2m_set_gate(b2m_ctx* ctx, int layer, const void* dev_gate_weight);
  * the layer (and by the look-ahead prediction made from the layer before it).  B2M_EINVAL for a layer out of range, a null
  * pointer, or a context whose router is not B2M_ROUTER_DEEPSEEK_V3. */
 int b2m_set_gate_bias(b2m_ctx* ctx, int layer, const float* dev_bias);
+/* B2M_ROUTER_QWEN_MOE with shared experts (Qwen2-MoE) only: the layer's shared_expert_gate.weight, [H] in the model dtype on
+ * the device.  Borrowed like the gate weight: it must stay valid, and is read by every forward or combine of the layer (a
+ * captured graph reads its contents at replay).  B2M_EINVAL for a layer out of range, a null pointer, a context whose router
+ * is not B2M_ROUTER_QWEN_MOE, or a context without shared experts. */
+int b2m_set_shared_gate(b2m_ctx* ctx, int layer, const void* dev_w);
 
 /* replaces: HostMemoryPool / cudaHostAlloc per node (core/memory/memory_pool.cpp:29-83) */
 int b2m_host_pin(b2m_ctx* ctx, void* host_ptr, size_t bytes);
@@ -303,7 +326,10 @@ int b2m_check_errors(b2m_ctx* ctx, void* stream);
 #define B2M_WS_HMID 7       /* dtype [T*k,I] */
 #define B2M_WS_Y 8          /* fp32  [T*k,H] */
 #define B2M_WS_SCORES 9     /* fp32  [T,E] softmax probabilities (B2M_ROUTER_DEEPSEEK_V3: unbiased sigmoid scores) */
-#define B2M_WS_LOGITS 10    /* router logits computed by the fused gate: model dtype (Mixtral) or fp32 */
+#define B2M_WS_LOGITS 10    /* router logits computed by the fused gate: model dtype (Mixtral, Qwen) or fp32 */
+#define B2M_WS_SHARED_GATE 11 /* dtype [T]   B2M_ROUTER_QWEN_MOE with shared experts: sigmoid(shared_expert_gate(x)), rounded
+                                 (B2M_ESTATE on other contexts) */
+#define B2M_WS_Y_SHARED 12  /* fp32  [T,H] shared-expert output (B2M_ESTATE on a context without shared experts) */
 int b2m_ws_ptr(b2m_ctx* ctx, int which, void** dev_ptr);
 
 /* replaces prefetch_handle.replace_cache_candidates(ids) (archer_prefetch_handle.cpp:195-205,

@@ -142,6 +142,7 @@ struct b2m_ctx {
   std::vector<const void*> gate_w;  // per layer device pointers
   std::vector<const float*> gate_bias;  // B2M_ROUTER_DEEPSEEK_V3: per layer e_score_correction_bias [E] (device, borrowed)
   std::vector<const uint16_t*> input_perm;  // B2M_WEIGHTS_INT4_G128_F16: per layer [E][H] gather table (device, borrowed) or null
+  std::vector<const void*> shared_gate_w;   // B2M_ROUTER_QWEN_MOE with shared experts: per layer [H] shared_expert_gate.weight
 
   // workspace
   int cap_T = 0, cap_R = 0;
@@ -159,6 +160,7 @@ struct b2m_ctx {
   float* d_y = nullptr;
   void* d_hmid_s = nullptr;
   float* d_y_s = nullptr;
+  void* d_shared_gate = nullptr;   // Qwen2-MoE: [T] model-dtype gate values of the shared expert
   int* h_counts = nullptr;  // pinned [E+1]
   bool last_counts_valid = false;
   CUtensorMap tm_xp[5], tm_hmid[5], tm_hmid_s[5];
@@ -808,7 +810,20 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
     make_int4_shape(&shape);
   }
-  if (cfg->router < 0 || cfg->router > 4) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router < 0 || cfg->router > 5) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router == B2M_ROUTER_QWEN_MOE) {
+    if (cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
+      return fail(nullptr, B2M_EINVAL, "qwen_moe router: experts are gate|up|down (expert_type %d), got expert_type %d",
+                  B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, cfg->expert_type);
+    if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16)
+      return fail(nullptr, B2M_EINVAL, "qwen_moe router: the model dtype must be bf16 or f16, got dtype %d", cfg->dtype);
+    if (cfg->n_group != 1 || cfg->topk_group != 1)
+      return fail(nullptr, B2M_EINVAL, "qwen_moe router: no group-limited routing (n_group=%d, topk_group=%d must be 1)",
+                  cfg->n_group, cfg->topk_group);
+    if (cfg->routed_scaling_factor != 1.0f)
+      return fail(nullptr, B2M_EINVAL, "qwen_moe router: weights are not scaled (routed_scaling_factor=%g must be 1.0)",
+                  (double)cfg->routed_scaling_factor);
+  }
   if (cfg->router == B2M_ROUTER_DEEPSEEK_V3) {
     if (cfg->n_group < 1 || cfg->n_group > 32 || cfg->num_experts % cfg->n_group)
       return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: n_group=%d must be in 1..32 and divide num_experts=%d", cfg->n_group,
@@ -907,6 +922,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   c->gate_w.assign(L, nullptr);
   c->gate_bias.assign(L, nullptr);
   c->input_perm.assign(L, nullptr);
+  c->shared_gate_w.assign(L, nullptr);
   CKC(cudaMalloc((void**)&c->d_slot_of, sizeof(int) * L * E));
   CKC(cudaMemset(c->d_slot_of, 0xff, sizeof(int) * L * E));
   CKC(cudaHostAlloc((void**)&c->h_stage, sizeof(int) * STAGE_RING * E, cudaHostAllocDefault));
@@ -947,6 +963,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
     CKC(cudaMalloc(&c->d_hmid_s, (size_t)T * cfg->shared_inter * esize));
     CKC(cudaMemset(c->d_hmid_s, 0, (size_t)T * cfg->shared_inter * esize));
     CKC(cudaMalloc((void**)&c->d_y_s, (size_t)T * H * sizeof(float)));
+    if (cfg->router == B2M_ROUTER_QWEN_MOE) CKC(cudaMalloc(&c->d_shared_gate, (size_t)T * esize));
   }
   for (int i = 0; tc && i < 5; ++i) {
     r = build_act_map(c, &c->tm_xp[i], c->d_xp, H, (int)R, NT_LIST[i]);
@@ -982,7 +999,7 @@ int b2m_ctx_destroy(b2m_ctx* c) {
   if (c->pk.base) cudaFree(c->pk.base);
   if (c->pk.d_ok) cudaFree(c->pk.d_ok);
   void* bufs[] = {c->d_slot_of, c->d_topk_idx, c->d_topk_w, c->d_row_of, c->d_perm_token, c->d_counts, c->d_offsets,
-                  c->d_chunk_counts, c->d_offsets_src, c->d_ticket, c->d_gbar, c->d_err, c->d_look, c->d_tl, c->d_dest_of, c->d_scores, c->d_logits, c->d_xp, c->d_hmid, c->d_y, c->d_hmid_s, c->d_y_s};
+                  c->d_chunk_counts, c->d_offsets_src, c->d_ticket, c->d_gbar, c->d_err, c->d_look, c->d_tl, c->d_dest_of, c->d_scores, c->d_logits, c->d_xp, c->d_hmid, c->d_y, c->d_hmid_s, c->d_y_s, c->d_shared_gate};
   for (void* b : bufs) if (b) cudaFree(b);
   for (int r = 0; r < c->p2p.nranks; ++r)
     if (c->p2p.peer_base[r] && r != c->p2p.rank) cudaIpcCloseMemHandle(c->p2p.peer_base[r]);
@@ -1077,6 +1094,18 @@ int b2m_set_gate_bias(b2m_ctx* c, int layer, const float* dev_bias) {
   return B2M_OK;
 }
 
+int b2m_set_shared_gate(b2m_ctx* c, int layer, const void* dev_w) {
+  int r = check_layer(c, layer);
+  if (r) return r;
+  if (c->cfg.router != B2M_ROUTER_QWEN_MOE)
+    return fail(c, B2M_EINVAL, "b2m_set_shared_gate: only a qwen_moe router (%d) has a shared-expert gate, this context's router is %d",
+                B2M_ROUTER_QWEN_MOE, c->cfg.router);
+  if (c->cfg.shared_inter <= 0) return fail(c, B2M_EINVAL, "b2m_set_shared_gate: the context has no shared experts (shared_inter = 0)");
+  if (!dev_w) return fail(c, B2M_EINVAL, "b2m_set_shared_gate: dev_w is null");
+  c->shared_gate_w[layer] = dev_w;
+  return B2M_OK;
+}
+
 int b2m_set_input_perm(b2m_ctx* c, int layer, const uint16_t* dev_perm) {
   int r = check_layer(c, layer);
   if (r) return r;
@@ -1160,6 +1189,14 @@ int b2m_ws_ptr(b2m_ctx* c, int which, void** p) {
     case B2M_WS_Y: *p = c->d_y; break;
     case B2M_WS_SCORES: *p = c->d_scores; break;
     case B2M_WS_LOGITS: *p = c->d_logits; break;
+    case B2M_WS_SHARED_GATE:
+      if (!c->d_shared_gate) return fail(c, B2M_ESTATE, "workspace %d: the context has no gated shared expert", which);
+      *p = c->d_shared_gate;
+      break;
+    case B2M_WS_Y_SHARED:
+      if (!c->d_y_s) return fail(c, B2M_ESTATE, "workspace %d: the context has no shared experts", which);
+      *p = c->d_y_s;
+      break;
     default: return fail(c, B2M_EINVAL, "unknown workspace id %d", which);
   }
   return B2M_OK;
@@ -1608,6 +1645,19 @@ int b2m_run_experts_ex(b2m_ctx* c, int layer, int T, int phases, void* stream) {
 
 static int run_shared(b2m_ctx* c, int layer, const void* x, int T, cudaStream_t st) {
   if (!c->shared_registered[layer]) return fail(c, B2M_ESTATE, "shared expert of layer %d not registered", layer);
+  if (c->d_shared_gate) {
+    // Qwen2-MoE: the gate values depend on x only, so they are computed here, ahead of the shared GEMMs on the same stream
+    if (!c->shared_gate_w[layer]) return fail(c, B2M_ESTATE, "layer %d has no shared-expert gate (b2m_set_shared_gate)", layer);
+    CombineParams g;
+    memset(&g, 0, sizeof g);
+    g.mode = COMBINE_QWEN_GATE;
+    g.x = x;
+    g.shared_gate_w = c->shared_gate_w[layer];
+    g.out = c->d_shared_gate;
+    g.T = T; g.H = c->cfg.hidden; g.k = c->cfg.top_k; g.dtype = c->cfg.dtype;
+    CK(c, launch_combine(g, st));
+    c->stats.kernel_launches += 1;
+  }
   const int nt = pick_nt(T);
   const int ks = pick_ksplit(c, T, c->cfg.hidden, c->cfg.shared_inter, 1, 1, nt);
   CUtensorMap tm_x;
@@ -1647,6 +1697,7 @@ static int combine_impl(b2m_ctx* c, int layer, const void* x, int T, void* out, 
   p.T = T; p.H = f.hidden; p.k = f.top_k; p.dtype = f.dtype;
   if (f.router == B2M_ROUTER_SWITCH_TOP1) p.mode = COMBINE_SWITCH;
   else if (f.numerics == B2M_NUMERICS_FP32) p.mode = COMBINE_FP32;
+  else if (f.router == B2M_ROUTER_QWEN_MOE) p.mode = COMBINE_QWEN;
   else p.mode = f.router == B2M_ROUTER_MIXTRAL ? COMBINE_MIXTRAL : COMBINE_DEEPSEEK;
   if (f.shared_inter > 0) {
     if (c->shared_in_flight) {
@@ -1658,6 +1709,7 @@ static int combine_impl(b2m_ctx* c, int layer, const void* x, int T, void* out, 
       if (r) return r;
     }
     p.y_shared = c->d_y_s;
+    p.shared_gate = reinterpret_cast<const uint16_t*>(c->d_shared_gate);
   }
   if (ep_collect) {
     p.ep_collect = 1;
@@ -1847,6 +1899,7 @@ static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
   if (c->fp8) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with fp8 weights");
   if (c->int4) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with int4 weights");
+  if (c->cfg.router == B2M_ROUTER_QWEN_MOE) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the qwen_moe router");
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
     return fail(c, B2M_EINVAL, "bad expert-parallel geometry (nranks=%d rank=%d cap=%d E=%d)", nranks, rank, cap, c->cfg.num_experts);
   if ((long long)nranks * cap > c->cap_R)

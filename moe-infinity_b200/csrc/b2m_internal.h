@@ -17,6 +17,7 @@ enum : int {
   ROUTER_DEEPSEEK_GROUP = 2,   // modeling_deepseek.py:484-505
   ROUTER_SWITCH_TOP1 = 3,      // HF 4.x SwitchTransformersTop1Router (switch_transformers.py:76)
   ROUTER_DEEPSEEK_V3 = 4,      // modeling_deepseek_v3/modeling_deepseek.py:466-527 (sigmoid, noaux_tc)
+  ROUTER_QWEN_MOE = 5,         // transformers Qwen2MoeTopKRouter / Qwen3MoeTopKRouter (model-dtype logits, fp32 weights)
 };
 // combine kinds (which reference combine loop is restated)
 enum : int {
@@ -24,6 +25,9 @@ enum : int {
   COMBINE_DEEPSEEK = 1,  // deepseek.py:123-128 (+133-136 shared experts); fp32 weights
   COMBINE_SWITCH = 2,    // switch_transformers.py:99-109
   COMBINE_FP32 = 3,      // fast path: fp32 accumulate, single rounding
+  COMBINE_QWEN = 4,      // Qwen2MoeExperts + Qwen2MoeSparseMoeBlock: product and += rounded, fp32 weights; gated shared expert
+  COMBINE_QWEN_GATE = 5, // the first phase of a Qwen2 combine, launched ahead of it on the shared-expert stream: out[t] =
+                         // sigmoid(x[t] . shared_gate_w) in the model dtype (x [T,H], shared_gate_w [H], out [T], 16-bit)
 };
 
 struct GemmParams {
@@ -223,7 +227,7 @@ cudaError_t launch_route_from_mask(const RouteParams& p, const uint8_t* mask /*[
 struct CombineParams {
   const float* y;          // [rows, H] fp32 expert outputs (permuted row order)
   const float* y_shared;   // [T, H] fp32 shared-expert output or null
-  const void* x;           // [T,H] (Switch pass-through) or null
+  const void* x;           // [T,H] (Switch pass-through; the COMBINE_QWEN_GATE input) or null
   const int* topk_idx;     // [T,k]
   const float* topk_w;     // [T,k]
   const int* row_of;       // [T,k]
@@ -233,6 +237,8 @@ struct CombineParams {
   int ep_early;            // direct mode: programmatic edge behind the down GEMM, no grid-completion wait (flags guard the data)
   EpParams ep;
   unsigned long long* tl;  // optional timeline slots: [0] start, [1] owners' flags seen, [2] end
+  const uint16_t* shared_gate;  // Qwen2-MoE: [T] model-dtype sigmoid(shared_expert_gate(x)) scaling y_shared (COMBINE_QWEN_GATE)
+  const void* shared_gate_w;    // COMBINE_QWEN_GATE: the layer's [H] shared_expert_gate.weight (model dtype)
 };
 cudaError_t launch_combine(const CombineParams& p, cudaStream_t st);
 cudaError_t launch_combine_f32(const CombineParams& p, cudaStream_t st);

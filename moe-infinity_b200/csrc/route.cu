@@ -31,6 +31,11 @@ __device__ __forceinline__ float load_as_float(const void* p, size_t i, int dt) 
 }
 // bytes of one hidden row of the model dtype (fp32 models: 4-byte elements; rows stay multiples of 16 B since H % 8 == 0)
 __device__ __forceinline__ size_t row_bytes(const RouteParams& p) { return (size_t)p.H * (p.dtype == DT_F32 ? 4 : 2); }
+// Routers whose gate is an nn.Linear in the model dtype: their logits are rounded to the model dtype before the softmax
+// (Mixtral, mixtral.py:46; Qwen2-MoE / Qwen3-MoE, modeling_qwen2_moe.py Qwen2MoeTopKRouter).  The others take fp32 logits.
+__host__ __device__ __forceinline__ bool logits_in_model_dtype(int router) {
+  return router == ROUTER_MIXTRAL || router == ROUTER_QWEN_MOE;
+}
 __device__ __forceinline__ float round_to(float f, int dt) {
   if (dt == DT_BF16) return round_dt<DT_BF16>(f);
   if (dt == DT_F16) return round_dt<DT_F16>(f);
@@ -97,7 +102,7 @@ __device__ float gate_dot_warp(const RouteParams& p, int t, int e) {
     }
   }
   acc = warp_sum(acc);
-  return (p.router == ROUTER_MIXTRAL) ? round_to(acc, p.dtype) : acc;
+  return logits_in_model_dtype(p.router) ? round_to(acc, p.dtype) : acc;
 }
 // One warp, one token, experts [e0, e0+8): x is loaded once per 8-element chunk and reused for all 8 rows
 // (16-byte loads of both operands).  out[i] (i < 8) valid in every lane.  No predicates inside the loop (expert
@@ -139,7 +144,7 @@ __device__ __forceinline__ void gate_dot8_impl(const RouteParams& p, int t, int 
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const float v = warp_sum(acc[i]);
-    out[i] = (p.router == ROUTER_MIXTRAL) ? round_to(v, p.dtype) : v;
+    out[i] = logits_in_model_dtype(p.router) ? round_to(v, p.dtype) : v;
   }
 }
 __device__ __forceinline__ void gate_dot8_warp(const RouteParams& p, int t, int e0, float (&out)[8]) {
@@ -258,7 +263,7 @@ __device__ __forceinline__ void gate_logits_impl(const RouteParams& p, uint4* ri
           const float v = warp_sum(acc[q][i]);
           const int t = t0 + q;
           if (lane == 0 && t < p.T && e0 + i < p.E) {
-            if (p.router == ROUTER_MIXTRAL)
+            if (logits_in_model_dtype(p.router))
               reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e0 + i] =
                   p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(v) : Half16<DT_F16>::from_f(v);
             else
@@ -487,6 +492,9 @@ __device__ void route_token_warp(const RouteParams& p, int t, const float* s_in 
       w = round_to(__fdiv_rn(sv, denom), p.dtype);                       // mixtral.py:52-54
     } else if (p.router == ROUTER_SWITCH_TOP1) {
       w = sv;
+    } else if (p.router == ROUTER_QWEN_MOE) {
+      // Qwen2MoeTopKRouter: fp32 weights, divided by their sum (selection order) for every k, no epsilon, no scaling
+      w = p.norm_topk_prob ? __fdiv_rn(sv, denom) : sv;
     } else if (p.k > 1 && p.norm_topk_prob) {
       w = __fdiv_rn(sv, __fadd_rn(denom, 1e-20f));                        // modeling_deepseek.py:508-510
     } else {
@@ -676,7 +684,7 @@ __global__ void __launch_bounds__(RT_THREADS) route_topk_kernel(const RouteParam
     if (p.logits_out && !scores_in) {
       for (int e = lane; e < p.E; e += 32) {
         const float lv = s_logits[warp][e];
-        if (p.router == ROUTER_MIXTRAL) {
+        if (logits_in_model_dtype(p.router)) {
           reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e] =
               p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(lv) : Half16<DT_F16>::from_f(lv);
         } else {
@@ -847,7 +855,7 @@ __global__ void __launch_bounds__(RT_THREADS) gate_topk_small_kernel(const Route
     if (p.logits_out && !scores_in) {
       for (int e = lane; e < p.E; e += 32) {
         const float lv = s_logits[e];
-        if (p.router == ROUTER_MIXTRAL)
+        if (logits_in_model_dtype(p.router))
           reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e] =
               p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(lv) : Half16<DT_F16>::from_f(lv);
         else
@@ -1100,7 +1108,7 @@ static bool route_args_ok(const RouteParams& p);
 // layer's input row and counts its top-k choice per expert.  softmax is monotonic, so top-k of the logits is the top-k of
 // the scores (ties -> lowest index, like every routing kernel here); weights are not needed for a prefetch hint.
 // DeepSeek-V3: the bias and the group rule change the order, so the next layer's full V3 selection runs (p.gate_bias =
-// that layer's bias).
+// that layer's bias).  Mixtral / Qwen: top-k of the logits rounded to the model dtype, as their routers rank them.
 __global__ void __launch_bounds__(RT_THREADS) lookahead_counts_kernel(const RouteParams p, int* __restrict__ counts_out) {
   __shared__ float s_logits[MAX_PL * 32];
   __shared__ float s_scr[MAX_PL * 32];
@@ -1188,7 +1196,7 @@ cudaError_t launch_route(const RouteParams& p, cudaStream_t st) {
       gate_logits_kernel<<<dim3(nblocks, gsplit), 256, 0, st>>>(p);
     }
     q.logits = p.logits_out;
-    q.logits_dtype = p.router == ROUTER_MIXTRAL ? p.dtype : DT_F32;
+    q.logits_dtype = logits_in_model_dtype(p.router) ? p.dtype : DT_F32;
     q.logits_are_scores = 0;
     q.logits_out = nullptr;
   }
@@ -1224,10 +1232,12 @@ cudaError_t launch_route_from_mask(const RouteParams& p, const uint8_t* mask, cu
 // K5: un-permute + weighted combine.  One warp-group of lanes shares a token's (row, weight) list by
 // warp shuffle; every lane owns 8 consecutive hidden elements (2 x 16 B fp32 loads per expert row,
 // one 16 B store).  Experts are applied in ascending expert id (the oracle's fixed order).
+// QWEN: the instantiation for Qwen2-MoE / Qwen3-MoE layers (COMBINE_QWEN, or COMBINE_FP32 with a gated shared expert); the
+// other instantiation compiles exactly the code it had before that mode existed.
 // --------------------------------------------------------------------------------------
 constexpr int CB_THREADS = 256;
 
-template <int DT>
+template <int DT, bool QWEN>
 __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams p) {
   const int t = blockIdx.x;
   const int lane = threadIdx.x & 31;
@@ -1342,6 +1352,11 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
               // out (model dtype) * weight (fp32) -> fp32; final(model dtype) += fp32 -> rounded (deepseek.py:125-128)
               const float prod = __fmul_rn(round_dt<DT>(y[i]), w);
               acc[i] = round_dt<DT>(__fadd_rn(acc[i], prod));
+            } else if (QWEN) {   // COMBINE_QWEN
+              // Qwen2MoeExperts: index_add_(final (model dtype, zeros), (out (model dtype) * weight (fp32)).to(model dtype)):
+              // the product is rounded, then every add is rounded
+              const float prod = round_dt<DT>(__fmul_rn(round_dt<DT>(y[i]), w));
+              acc[i] = round_dt<DT>(__fadd_rn(acc[i], prod));
             } else {  // COMBINE_SWITCH: next_states[idx] = out (switch_transformers.py:99-101)
               acc[i] = round_dt<DT>(y[i]);
             }
@@ -1365,10 +1380,21 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
       const float4* src = reinterpret_cast<const float4*>(p.y_shared + (size_t)t * H + h);
       const float4 a = src[0], b = src[1];
       const float s[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+      if (QWEN) {
+        // Qwen2MoeSparseMoeBlock: out + sigmoid(shared_expert_gate(x)) * shared_expert(x), every op in the model dtype;
+        // g = that sigmoid, already rounded (shared_gate_kernel)
+        const float g = Half16<DT>::to_f(p.shared_gate[t]);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        if (p.mode == COMBINE_FP32) acc[i] += s[i];
-        else acc[i] = round_dt<DT>(__fadd_rn(acc[i], round_dt<DT>(s[i])));   // final + shared_experts(identity), deepseek.py:133-136
+        for (int i = 0; i < 8; ++i) {
+          if (p.mode == COMBINE_FP32) acc[i] = fmaf(g, s[i], acc[i]);
+          else acc[i] = round_dt<DT>(__fadd_rn(acc[i], round_dt<DT>(__fmul_rn(g, round_dt<DT>(s[i])))));
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          if (p.mode == COMBINE_FP32) acc[i] += s[i];
+          else acc[i] = round_dt<DT>(__fadd_rn(acc[i], round_dt<DT>(s[i])));   // final + shared_experts(identity), deepseek.py:133-136
+        }
       }
     }
     uint4 o;
@@ -1380,16 +1406,65 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
 }
 
+static cudaError_t launch_shared_gate(const CombineParams& p, cudaStream_t st);
+
 cudaError_t launch_combine(const CombineParams& p, cudaStream_t st) {
   if (p.T == 0) return cudaSuccess;
+  if (p.mode == COMBINE_QWEN_GATE) return launch_shared_gate(p, st);
   if (p.k > MAX_K || p.H % 8 != 0) return cudaErrorInvalidValue;
   int gy = (p.H + CB_THREADS * 8 - 1) / (CB_THREADS * 8);
   dim3 grid(p.T, gy);
   if (p.dtype == DT_F32) return launch_combine_f32(p, st);
   const bool early = p.ep_collect && p.ep.direct && p.ep_early;
-  if (p.dtype == DT_BF16) return launch_cluster(combine_kernel<DT_BF16>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
-  if (p.dtype == DT_F16) return launch_cluster(combine_kernel<DT_F16>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
+  const bool qwen = p.mode == COMBINE_QWEN || p.shared_gate;
+  if (qwen && (p.ep_collect || (p.y_shared && !p.shared_gate))) return cudaErrorInvalidValue;
+  if (p.dtype == DT_BF16)
+    return qwen ? launch_cluster(combine_kernel<DT_BF16, true>, grid, dim3(CB_THREADS), 0, st, 1, false, p)
+                : launch_cluster(combine_kernel<DT_BF16, false>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
+  if (p.dtype == DT_F16)
+    return qwen ? launch_cluster(combine_kernel<DT_F16, true>, grid, dim3(CB_THREADS), 0, st, 1, false, p)
+                : launch_cluster(combine_kernel<DT_F16, false>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
   return cudaErrorInvalidValue;
+}
+
+// --------------------------------------------------------------------------------------
+// Qwen2-MoE shared-expert gate: g[t] = sigmoid(shared_expert_gate(x[t])) with every op in the model dtype (an nn.Linear(H, 1)
+// without bias, then F.sigmoid): the dot is accumulated in fp32 and rounded, the sigmoid is PyTorch's CUDA formula on that
+// value (sigmoid_ref, as the V3 router) and is rounded again.  One warp per token, 16-byte loads of both operands.  It
+// depends on x only: launch_combine runs it as the COMBINE_QWEN_GATE phase, which the caller issues on the shared-expert
+// stream beside the routing kernels; the combine proper reads g.
+// --------------------------------------------------------------------------------------
+template <int DT>
+__global__ void __launch_bounds__(256) shared_gate_kernel(const uint16_t* __restrict__ x, const uint16_t* __restrict__ w,
+                                                          uint16_t* __restrict__ out, int T, int H) {
+  const int lane = threadIdx.x & 31;
+  const int t = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (t >= T) return;
+  const uint16_t* xr = x + (size_t)t * H;
+  float acc = 0.f;
+  for (int h = lane * 8; h < H; h += 256) {
+    float xf[8], wf[8];
+    unpack8(*reinterpret_cast<const uint4*>(xr + h), DT, xf);
+    unpack8(*reinterpret_cast<const uint4*>(w + h), DT, wf);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc = fmaf(xf[j], wf[j], acc);
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) out[t] = Half16<DT>::from_f(round_dt<DT>(sigmoid_ref(round_dt<DT>(acc))));
+}
+
+static cudaError_t launch_shared_gate(const CombineParams& p, cudaStream_t st) {
+  const int T = p.T, H = p.H;
+  if (T < 0 || H % 8 || !p.x || !p.shared_gate_w || !p.out) return cudaErrorInvalidValue;
+  const dim3 grid((T + 7) / 8);
+  const uint16_t* xs = reinterpret_cast<const uint16_t*>(p.x);
+  const uint16_t* ws = reinterpret_cast<const uint16_t*>(p.shared_gate_w);
+  uint16_t* o = reinterpret_cast<uint16_t*>(p.out);
+  const int dtype = p.dtype;
+  if (dtype == DT_BF16) shared_gate_kernel<DT_BF16><<<grid, 256, 0, st>>>(xs, ws, o, T, H);
+  else if (dtype == DT_F16) shared_gate_kernel<DT_F16><<<grid, 256, 0, st>>>(xs, ws, o, T, H);
+  else return cudaErrorInvalidValue;
+  return cudaGetLastError();
 }
 
 template <int DT>

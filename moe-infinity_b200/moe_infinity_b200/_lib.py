@@ -15,11 +15,13 @@ STORE_NO_ODIRECT = 1
 DTYPE_BF16, DTYPE_F32, DTYPE_F16, DTYPE_FP8 = 0, 1, 2, 3
 EXPERT_SWITCH, EXPERT_SWITCH_GATED, EXPERT_NLLB, EXPERT_FSGPT, EXPERT_MIXTRAL, EXPERT_DEEPSEEK = 0, 1, 2, 3, 4, 5
 ROUTER_MIXTRAL, ROUTER_DEEPSEEK_GREEDY, ROUTER_DEEPSEEK_GROUP, ROUTER_SWITCH_TOP1, ROUTER_DEEPSEEK_V3 = 0, 1, 2, 3, 4
+ROUTER_QWEN_MOE = 5
 NUMERICS_REFERENCE, NUMERICS_FP32 = 0, 1
 CACHE_REFERENCE, CACHE_SLOTS, CACHE_ACTIVATION_AWARE = 0, 1, 2
 WEIGHTS_MODEL_DTYPE, WEIGHTS_FP8_E4M3_B128 = 0, 1
 WEIGHTS_INT4_G128, WEIGHTS_INT4_G128_F16 = 4, 6
-WS = dict(topk_idx=0, topk_w=1, row_of=2, perm_token=3, counts=4, offsets=5, xp=6, hmid=7, y=8, scores=9, logits=10)
+WS = dict(topk_idx=0, topk_w=1, row_of=2, perm_token=3, counts=4, offsets=5, xp=6, hmid=7, y=8, scores=9, logits=10,
+          shared_gate=11, y_shared=12)
 
 
 class Config(C.Structure):
@@ -57,6 +59,7 @@ SYMBOLS = [
     ("b2m_set_gate", _I, [_VP, _I, _VP]),
     ("b2m_set_gate_bias", _I, [_VP, _I, _VP]),
     ("b2m_set_input_perm", _I, [_VP, _I, _VP]),
+    ("b2m_set_shared_gate", _I, [_VP, _I, _VP]),
     ("b2m_host_pin", _I, [_VP, _VP, _SZ]),
     ("b2m_host_unpin", _I, [_VP, _VP]),
     ("b2m_make_resident", _I, [_VP, _I, _I, _I, _VP]),

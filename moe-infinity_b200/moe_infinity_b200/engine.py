@@ -75,7 +75,8 @@ class MoEEngine:
         self.shared_inter = shared_inter
         self.expert_type = expert_type
         self.router = router
-        gate_dtype = gate_dtype or (dtype if router == L.ROUTER_MIXTRAL else torch.float32)
+        # Mixtral and Qwen routers are nn.Linear layers of the model: their weight is in the model dtype
+        gate_dtype = gate_dtype or (dtype if router in (L.ROUTER_MIXTRAL, L.ROUTER_QWEN_MOE) else torch.float32)
         self.gate_dtype = gate_dtype
         cfg = L.Config()
         cfg.struct_size = C.sizeof(L.Config)
@@ -111,6 +112,7 @@ class MoEEngine:
         self._gates: Dict[int, torch.Tensor] = {}
         self._biases: Dict[int, torch.Tensor] = {}
         self._perms: Dict[int, torch.Tensor] = {}
+        self._shared_gates: Dict[int, torch.Tensor] = {}
         es = self.esize = 4 if dtype == torch.float32 else 2   # fp32 experts (dtype int 1) run on the CUDA-core fp32 path
         if expert_type in (L.EXPERT_NLLB, L.EXPERT_FSGPT):     # fc1 | fc1_bias | fc2 | fc2_bias (expert_module.cpp:70-77)
             self.expert_bytes = 2 * hidden * inter * es + (inter + hidden) * es
@@ -303,6 +305,18 @@ class MoEEngine:
         self._biases[layer] = b                # borrowed by the context: keep it alive
         self._ck(self.lib.b2m_set_gate_bias(self._h, layer, C.c_void_p(b.data_ptr())))
 
+    def set_shared_gate(self, layer: int, weight: torch.Tensor):
+        """Qwen2-MoE (router=ROUTER_QWEN_MOE with shared_inter > 0): the layer's shared_expert_gate.weight, [1, H] or [H] in
+        the model dtype.  The combine scales the shared expert's output by sigmoid(x . weight), every op in the model dtype."""
+        if self.router != L.ROUTER_QWEN_MOE or self.shared_inter <= 0:
+            raise ValueError("set_shared_gate needs a Qwen-MoE engine with shared experts (router=ROUTER_QWEN_MOE, shared_inter > 0)")
+        if weight.dtype != self.dtype or tuple(weight.shape) not in ((1, self.H), (self.H,)):
+            raise ValueError(f"expected a {self.dtype} [1, {self.H}] or [{self.H}] shared-expert gate, got {weight.dtype} "
+                             f"{tuple(weight.shape)}")
+        w = weight.detach().reshape(self.H).to(self.device).contiguous()
+        self._shared_gates[layer] = w          # borrowed by the context: keep it alive
+        self._ck(self.lib.b2m_set_shared_gate(self._h, layer, C.c_void_p(w.data_ptr())))
+
     def set_input_perm(self, layer: int, perm: Optional[torch.Tensor]):
         """Act-order GPTQ on an f16 int4 engine (B2M_WEIGHTS_INT4_G128_F16): perm int [E, H], row e a permutation of
         0..H-1 (`int4.from_gptq_act_order`); the routing kernels gather column j of expert e's rows from x[t][perm[e][j]],
@@ -388,12 +402,13 @@ class MoEEngine:
         p = C.c_void_p()
         self._ck(self.lib.b2m_ws_ptr(self._h, L.WS[name], C.byref(p)))
         k, E, H, I = self.k, self.E, self.H, self.I
-        logits_dt = self.dtype if self.router == L.ROUTER_MIXTRAL else torch.float32
+        logits_dt = self.dtype if self.router in (L.ROUTER_MIXTRAL, L.ROUTER_QWEN_MOE) else torch.float32
         shape, dt = {
             "topk_idx": ((T, k), torch.int32), "topk_w": ((T, k), torch.float32), "row_of": ((T, k), torch.int32),
             "perm_token": ((T * k,), torch.int32), "counts": ((E,), torch.int32), "offsets": ((E + 1,), torch.int32),
             "xp": ((T * k, H), self.dtype), "hmid": ((T * k, I), self.dtype), "y": ((T * k, H), torch.float32),
             "scores": ((T, E), torch.float32), "logits": ((T, E), logits_dt),
+            "shared_gate": ((T,), self.dtype), "y_shared": ((T, H), torch.float32),
         }[name]
         return _view(p.value, shape, dt, self.device)
 

@@ -1,5 +1,5 @@
-"""HuggingFace plug-in helpers: run a `transformers` Mixtral or DeepSeek-V3 model with its MoE blocks executed by the CUDA
-engine (`patch_mixtral`, `patch_deepseek_v3`), and load the routed experts of a published AWQ / GPTQ 4-bit checkpoint into
+"""HuggingFace plug-in helpers: run a `transformers` Mixtral, DeepSeek-V3, Qwen2-MoE or Qwen3-MoE model with its MoE blocks
+executed by the CUDA engine (`patch_mixtral`, `patch_deepseek_v3`, `patch_qwen_moe`), and load the routed experts of a published AWQ / GPTQ 4-bit checkpoint into
 an f16 int4 engine as they are stored (`load_int4_checkpoint`).
 
 The reference achieves this by monkey-patching HF classes at load time (moe_infinity/runtime/model_offload.py:285-321:
@@ -135,6 +135,70 @@ def patch_deepseek_v3(model, max_tokens: int = 4096, num_slots: int = 0, device_
     return engine
 
 
+class B200QwenMoeAdapter(nn.Module):
+    """Drop-in for transformers>=5 `Qwen2MoeSparseMoeBlock` / `Qwen3MoeSparseMoeBlock`: forward(hidden[B,S,H]) ->
+    hidden[B,S,H].  The router GEMM stays in PyTorch (`F.linear` in the model dtype, the logits HF's Qwen2MoeTopKRouter
+    computes); the softmax, top-k, weights, routed experts, gated shared expert (Qwen2) and the combine run in the engine."""
+
+    def __init__(self, engine: MoEEngine, layer_id: int, gate_weight: torch.Tensor):
+        super().__init__()
+        self.engine = engine
+        self.layer_id = layer_id
+        self.gate_weight = nn.Parameter(gate_weight.detach().clone(), requires_grad=False)
+
+    def forward(self, hidden_states: torch.Tensor) -> torch.Tensor:
+        shape = hidden_states.shape
+        x = hidden_states.reshape(-1, shape[-1])
+        router_logits = F.linear(x, self.gate_weight)
+        out = self.engine.forward(self.layer_id, x, router_logits=router_logits)
+        return out.reshape(shape)
+
+
+def _is_qwen_sparse_block(mlp) -> bool:
+    return hasattr(mlp, "experts") and hasattr(mlp, "gate") and hasattr(mlp.experts, "gate_up_proj")
+
+
+def patch_qwen_moe(model, max_tokens: int = 4096, num_slots: int = 0, device_memory_ratio: float = 0.0,
+                   resident: bool = True, engine: Optional[MoEEngine] = None) -> MoEEngine:
+    """Move the routed experts, shared experts and shared-expert gates (Qwen2-MoE) of `model` (a transformers
+    Qwen2MoeForCausalLM or Qwen3MoeForCausalLM, or their base models, on a CUDA device) into a MoEEngine
+    (ROUTER_QWEN_MOE, gate|up|down experts) and replace its sparse MoE blocks.  Only layers whose `mlp` is the sparse block
+    are replaced, so `mlp_only_layers` and `decoder_sparse_step` keep their dense MLPs.  `engine` may be given (built with
+    router=ROUTER_QWEN_MOE and the model's shapes), e.g. one with expert_dtype=torch.float8_e4m3fn or torch.uint4: the
+    routed experts are then quantised with `fp8.quantize_block128` or `int4.quantize_g128`; shared experts stay in the
+    model dtype.  `resident=False` registers the routed experts as pinned host blobs (offload mode, budget from num_slots /
+    device_memory_ratio)."""
+    cfg = model.config
+    layers = model.model.layers if hasattr(model, "model") else model.layers
+    dev = next(model.parameters()).device
+    dtype = next(model.parameters()).dtype
+    L_, E, H, I, k = len(layers), cfg.num_experts, cfg.hidden_size, cfg.moe_intermediate_size, cfg.num_experts_per_tok
+    moe_layers = [l for l in range(L_) if _is_qwen_sparse_block(layers[l].mlp)]
+    shared = bool(moe_layers) and hasattr(layers[moe_layers[0]].mlp, "shared_expert")
+    shared_inter = cfg.shared_expert_intermediate_size if shared else 0
+    if engine is None:
+        engine = MoEEngine(num_layers=L_, num_experts=E, hidden=H, inter=I, top_k=k, dtype=dtype, expert_type=L.EXPERT_DEEPSEEK,
+                           router=L.ROUTER_QWEN_MOE, max_tokens=max_tokens,
+                           num_slots=(L_ * E if resident and not num_slots else num_slots),
+                           device_memory_ratio=device_memory_ratio, shared_inter=shared_inter,
+                           norm_topk_prob=bool(cfg.norm_topk_prob), device=dev.index or 0)
+    elif engine.router != L.ROUTER_QWEN_MOE or engine.expert_type != L.EXPERT_DEEPSEEK:
+        raise ValueError("patch_qwen_moe needs an engine built with router=ROUTER_QWEN_MOE and expert_type=EXPERT_DEEPSEEK")
+    elif engine.shared_inter != shared_inter:
+        raise ValueError(f"the engine's shared_inter {engine.shared_inter} does not match the model's {shared_inter}")
+    for l in moe_layers:
+        moe = layers[l].mlp
+        gu, dn = moe.experts.gate_up_proj.data, moe.experts.down_proj.data     # [E,2I,H], [E,H,I]
+        for e in range(E):
+            _load(engine, l, e, [gu[e, :I], gu[e, I:], dn[e]], resident)     # HF order: gate | up | down
+        if shared:
+            sh = moe.shared_expert
+            engine.register_shared(l, [sh.gate_proj.weight.data, sh.up_proj.weight.data, sh.down_proj.weight.data])
+            engine.set_shared_gate(l, moe.shared_expert_gate.weight.data)
+        layers[l].mlp = B200QwenMoeAdapter(engine, l, moe.gate.weight.data)
+    return engine
+
+
 # ---------------------------------------------------------------- published AWQ / GPTQ checkpoints
 def _int4_method(qc: dict) -> str:
     """Validate a checkpoint's `quantization_config` and return "awq", "gptq" or "gptq_v2"."""
@@ -163,14 +227,18 @@ def _int4_method(qc: dict) -> str:
 def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], quantization_config: dict, model_type: str,
                          resident: bool = True, act_order: bool = False) -> List[int]:
     """Load the routed experts and router weights of a published AWQ or GPTQ 4-bit checkpoint (its safetensors `shards`,
-    its config's `quantization_config`, `model_type` "mixtral" or "deepseek_v2" / "deepseek_v3") into `engine`, an int4
+    its config's `quantization_config`, `model_type` "mixtral", "deepseek_v2" / "deepseek_v3" or "qwen2_moe" / "qwen3_moe")
+    into `engine`, an int4
     engine with float16 activations (`MoEEngine(dtype=torch.float16, expert_dtype=torch.uint4)`), without changing a
     weight (`int4.from_awq` / `int4.from_gptq`).  Tensors are read one at a time with `safetensors.safe_open`.
 
     Mixtral: model.layers.{l}.block_sparse_moe.experts.{e}.w{1,2,3}.* and ...block_sparse_moe.gate.weight.  DeepSeek:
     model.layers.{l}.mlp.experts.{e}.{gate,up,down}_proj.*, mlp.gate.weight (and mlp.gate.e_score_correction_bias for a V3
     router) and mlp.shared_experts.*, whose dequantised weights are registered as the f16 shared expert; layers without
-    experts (no mlp.gate.weight) are skipped.  `resident=False` registers the experts as pinned host blobs (offload).
+    experts (no mlp.gate.weight) are skipped.  Qwen2-MoE / Qwen3-MoE (an engine with router=ROUTER_QWEN_MOE): the same
+    routed-expert and router names, mlp.shared_expert.{gate,up,down}_proj.* for the shared expert (dequantised to f16) and
+    the plain mlp.shared_expert_gate.weight for its gate (a checkpoint holding only a quantised form of that gate is
+    refused).  `resident=False` registers the experts as pinned host blobs (offload).
     act_order=True loads act-order GPTQ (desc_act, a g_idx other than c // 128) as well, without changing a weight: per
     expert, P = the gate/up order and P2 = the down projection's (`int4.from_gptq_act_order`); the engine stores
     gate/up as W[P2][:, P] and down as W[:, P2] (so the gate/up GEMM writes h[P2], which the down projection consumes),
@@ -186,10 +254,14 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
                          "(MoEEngine(dtype=torch.float16, expert_dtype=torch.uint4))")
     method = _int4_method(quantization_config)
     mixtral = model_type == "mixtral"
-    if not mixtral and not model_type.startswith("deepseek"):
-        raise ValueError(f"model_type {model_type!r}: Mixtral and DeepSeek checkpoints are supported")
+    qwen = model_type in ("qwen2_moe", "qwen3_moe")
+    if not mixtral and not qwen and not model_type.startswith("deepseek"):
+        raise ValueError(f"model_type {model_type!r}: Mixtral, DeepSeek and Qwen-MoE checkpoints are supported")
     if mixtral != (engine.expert_type == L.EXPERT_MIXTRAL):
         raise ValueError(f"model_type {model_type!r} does not match the engine's expert_type {engine.expert_type}")
+    if qwen != (engine.router == L.ROUTER_QWEN_MOE):
+        raise ValueError(f"model_type {model_type!r} does not match the engine's router {engine.router}")
+    shared_name = "shared_expert" if qwen else "shared_experts"
     if isinstance(shards, str):
         shards = [shards]
     parts = ("qweight", "qzeros", "scales")
@@ -236,7 +308,13 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
             need.append(f"{base}.gate.weight")
             need += [f"{base}.experts.{e}.{n}.{p}" for e in range(engine.E) for n in names for p in parts]
             if not mixtral and engine.shared_inter > 0:
-                need += [f"{base}.shared_experts.{n}.{p}" for n in names for p in parts]
+                need += [f"{base}.{shared_name}.{n}.{p}" for n in names for p in parts]
+            if qwen and engine.shared_inter > 0:
+                key = f"{base}.shared_expert_gate"
+                if f"{key}.weight" not in where and f"{key}.qweight" in where:
+                    raise ValueError(f"the checkpoint stores {key} quantised ({key}.qweight); its plain {key}.weight "
+                                     "is needed (the shared-expert gate runs in the model dtype)")
+                need.append(f"{key}.weight")
             if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:
                 need.append(f"{base}.gate.e_score_correction_bias")
         missing = [k for k in need if k not in where]
@@ -265,7 +343,10 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
             if act_order and not torch.equal(table, torch.arange(engine.H).expand(engine.E, engine.H)):
                 engine.set_input_perm(l, table)
             if not mixtral and engine.shared_inter > 0:
-                engine.register_shared(l, [shared(f"{base}.shared_experts.{n}") for n in names])
+                engine.register_shared(l, [shared(f"{base}.{shared_name}.{n}") for n in names])
+            if qwen and engine.shared_inter > 0:
+                key = f"{base}.shared_expert_gate.weight"
+                engine.set_shared_gate(l, where[key].get_tensor(key).to(engine.dtype))
             key = f"{base}.gate.weight"
             engine.set_gate(l, where[key].get_tensor(key))
             if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:
