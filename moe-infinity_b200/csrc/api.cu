@@ -78,9 +78,26 @@ struct ExpertShape {
   size_t off_gate = 0, off_up = 0, off_down = 0, bytes = 0;
   bool has_bias = false;          // fc1 | fc1_bias | fc2 | fc2_bias (NLLB / FSGPT)
   size_t off_bias1 = 0, off_bias2 = 0;
-  bool fp8 = false;               // e4m3 matrices + fp32 128x128 block-scale grids (fp8_weights.cuh)
-  bool int4 = false;              // 4-bit code matrices + tile-major group grids (int4_weights.cuh)
-  size_t sc_gate = 0, sc_up = 0, sc_down = 0;   // fp8 / int4: byte offsets of the three scale / group grids
+  int bits = 16;                  // bits per stored weight
+  size_t grid_gate = 0, grid_up = 0, grid_down = 0;   // quantised formats: byte offsets of the matrices' side grids
+};
+
+// How routed experts are stored: one row per B2M_WEIGHTS_* value.  A quantised format's header (fp8_weights.cuh,
+// int4_weights.cuh) defines its blob and decode; gemm_body in grouped_gemm.cu decodes it for its A source.
+struct WeightFormat {
+  int id;                               // B2M_WEIGHTS_*
+  const char* name;                     // in messages
+  int act_dtype;                        // the model dtype (activations) the format needs; -1 = any
+  int bits;                             // bits per stored weight; 0 = the model dtype's
+  size_t (*grid_bytes)(int H, int I);   // bytes of one matrix's side grid (block scales / group words); null = none
+  int hi_multiple;                      // hidden and inter must be multiples of this
+  int a_src;                            // AS_*: how the tensor-core GEMMs read the weights
+};
+const WeightFormat WEIGHT_FORMATS[] = {
+    {B2M_WEIGHTS_MODEL_DTYPE, "model-dtype", -1, 0, nullptr, 1, AS_BF16},
+    {B2M_WEIGHTS_FP8_E4M3_B128, "fp8", B2M_DTYPE_BF16, 8, f8::scale_grid_bytes, f8::BLOCK, AS_FP8},
+    {B2M_WEIGHTS_INT4_G128, "int4", B2M_DTYPE_BF16, 4, i4::grid_bytes, i4::GROUP, AS_INT4},
+    {B2M_WEIGHTS_INT4_G128_F16, "int4 (fp16 scales)", B2M_DTYPE_F16, 4, i4::grid_bytes, i4::GROUP, AS_INT4},
 };
 
 struct Arena {
@@ -187,8 +204,7 @@ struct b2m_ctx {
   std::vector<int> last_active;
 
   int cur_ksplit = 1, cur_nt = 16, cur_nt_dn = 16, cur_T = 0;   // token-tile widths of the up (K3) and down (K4) GEMMs
-  bool fp8 = false;           // routed experts in B2M_WEIGHTS_FP8_E4M3_B128 (arena.shape.fp8)
-  bool int4 = false;          // routed experts in B2M_WEIGHTS_INT4_G128 or _F16 (arena.shape.int4; the scales' type is cfg.dtype)
+  const WeightFormat* wf = nullptr;   // how the routed experts are stored
   bool ep_mode = false;       // experts of other ranks are simply absent (never an error)
   // 12-bit packed copy of the routed arena (weight_pack.cuh; same slot index), read by the decode GEMMs.  Allocated by the first
   // eager forward that packs, if the device keeps PK_RESERVE free beside it.  d_ok[slot]: bit b = matrix b (gate, up, down)
@@ -275,72 +291,59 @@ int fail(b2m_ctx* c, int code, const char* fmt, ...) {
       return fail((c), B2M_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
-bool make_shape(int expert_type, int H, int I, ExpertShape* s, size_t esize = 2) {
-  const size_t m = (size_t)H * I * esize;
+// Slot layout of one expert: its matrices in the model's tensor order, H * I * bits / 8 bytes each, then (quantised formats)
+// one side grid of grid_bytes per matrix in the same order; rounded up to 16 B so that TMA strides stay multiples of 16 B.
+// For fp8 and int4 this is f8::expert_blob_bytes / i4::expert_blob_bytes.
+bool make_shape(int expert_type, int H, int I, int bits, size_t grid_bytes, ExpertShape* s) {
+  const size_t m = (size_t)H * I * bits / 8, esize = bits / 8;
   s->H = H;
   s->I = I;
+  s->bits = bits;
   switch (expert_type) {
     case B2M_EXPERT_MIXTRAL_MOE_DENSE_ACT_DENSE:  // w1 | w2 | w3  (expert_module.cpp:139-145)
       s->dual = true; s->act = ACT_SILU; s->off_gate = 0; s->off_down = m; s->off_up = 2 * m; s->bytes = 3 * m;
-      return true;
+      break;
     case B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE:  // gate | up | down  (:185-191)
       s->dual = true; s->act = ACT_SILU; s->off_gate = 0; s->off_up = m; s->off_down = 2 * m; s->bytes = 3 * m;
-      return true;
+      break;
     case B2M_EXPERT_SWITCH_DENSE_GATED_ACT_DENSE:  // wi_0 | wi_1 | wo  (:45-52)
       s->dual = true; s->act = ACT_GELU; s->off_gate = 0; s->off_up = m; s->off_down = 2 * m; s->bytes = 3 * m;
-      return true;
+      break;
     case B2M_EXPERT_SWITCH_DENSE_ACT_DENSE:  // wi | wo  (:17-23)
       s->dual = false; s->act = ACT_RELU; s->off_gate = 0; s->off_up = 0; s->off_down = m; s->bytes = 2 * m;
-      return true;
+      break;
     case B2M_EXPERT_NLLB_MOE_DENSE_ACT_DENSE:   // fc1 | fc1_bias | fc2 | fc2_bias  (:70-77; forward :88-92)
     case B2M_EXPERT_FSGPT_MOE_DENSE_ACT_DENSE:  // same binding (:104-111; forward :124-128, ReLU as well)
       s->dual = false; s->act = ACT_RELU; s->has_bias = true;
       s->off_gate = 0; s->off_up = 0; s->off_bias1 = m; s->off_down = m + (size_t)I * esize;
       s->off_bias2 = s->off_down + m; s->bytes = s->off_bias2 + (size_t)H * esize;   // H, I multiples of 8: all 16-B aligned
-      return true;
+      break;
     default:
       return false;
   }
+  if (grid_bytes) {
+    s->grid_gate = 3 * m + s->off_gate / m * grid_bytes;
+    s->grid_up = 3 * m + s->off_up / m * grid_bytes;
+    s->grid_down = 3 * m + s->off_down / m * grid_bytes;
+    s->bytes += 3 * grid_bytes;
+  }
+  s->bytes = (s->bytes + 15) & ~(size_t)15;
+  return true;
 }
 
-// routed experts of an fp8 context: the model's matrices as e4m3 bytes, then their scale grids (fp8_weights.cuh)
-void make_fp8_shape(ExpertShape* s) {
-  s->fp8 = true;
-  s->sc_gate = f8::scale_grid_offset(s->H, s->I, s->off_gate);
-  s->sc_up = f8::scale_grid_offset(s->H, s->I, s->off_up);
-  s->sc_down = f8::scale_grid_offset(s->H, s->I, s->off_down);
-  s->bytes = f8::expert_blob_bytes(s->H, s->I);
-}
-
-// routed experts of an int4 context: the model's matrices as 4-bit codes, then their group grids (int4_weights.cuh).  make_shape
-// ran with one-byte elements, so off_* / (H * I) is each matrix's place in the blob.
-void make_int4_shape(ExpertShape* s) {
-  const size_t m = (size_t)s->H * (size_t)s->I;
-  const int ig = (int)(s->off_gate / m), iu = (int)(s->off_up / m), id = (int)(s->off_down / m);
-  s->int4 = true;
-  s->off_gate = i4::code_offset(s->H, s->I, ig);
-  s->off_up = i4::code_offset(s->H, s->I, iu);
-  s->off_down = i4::code_offset(s->H, s->I, id);
-  s->sc_gate = i4::grid_offset(s->H, s->I, ig);
-  s->sc_up = i4::grid_offset(s->H, s->I, iu);
-  s->sc_down = i4::grid_offset(s->H, s->I, id);
-  s->bytes = i4::expert_blob_bytes(s->H, s->I);
-}
-
-// tensor-map element kind of the int4 code matrices (uint8 elements, 32-byte rows, SWIZZLE_32B: int4_weights.cuh)
-constexpr int MAP_INT4_CODES = -4;
-// dtype B2M_DTYPE_FP8_E4M3: e4m3 matrices as uint8 elements, 64-byte rows (SWIZZLE_64B, fp8_weights.cuh)
-int encode_map(b2m_ctx* c, CUtensorMap* tm, int dtype, void* base, int rank, const uint64_t* dims,
+// A K-major tensor map over `bits`-bit values: 16-bit values in the model dtype, narrower ones as uint8 bytes.  One k-row of
+// the GEMM's 64-wide k-block spans 64 * bits / 8 bytes (128, 64 or 32), and that span is the swizzle.
+int encode_map(b2m_ctx* c, CUtensorMap* tm, int bits, void* base, int rank, const uint64_t* dims,
                const uint64_t* strides_bytes /*rank-1*/, const uint32_t* box) {
   cuuint64_t gdim[3];
   cuuint64_t gstr[2];
   cuuint32_t b[3], es[3];
   for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; b[i] = box[i]; es[i] = 1; }
   for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
-  const bool u4 = dtype == MAP_INT4_CODES, u8 = dtype == B2M_DTYPE_FP8_E4M3 || u4;
-  CUtensorMapDataType dt = u8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
-                         : dtype == B2M_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapSwizzle swz = u4 ? CU_TENSOR_MAP_SWIZZLE_32B : u8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+  const CUtensorMapDataType dt = bits < 16 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                               : c->cfg.dtype == B2M_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const int span = 64 * bits / 8;
+  const CUtensorMapSwizzle swz = span == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : span == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
   CUresult r = c->encode(tm, dt, (cuuint32_t)rank, base, gdim, gstr, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -356,24 +359,21 @@ int build_arena_maps(b2m_ctx* c, Arena* a) {
 }
 int build_arena_maps_box(b2m_ctx* c, Arena* a, uint32_t box_rows, CUtensorMap* tg, CUtensorMap* tu, CUtensorMap* td) {
   const ExpertShape& s = a->shape;
-  // 64 k: the GEMM's k-block for every element size (int4: 32 bytes of two codes each)
-  const uint32_t box[3] = {s.int4 ? (uint32_t)i4::ROW_BYTES : 64u, box_rows, 1};
-  const int dt = s.int4 ? MAP_INT4_CODES : s.fp8 ? B2M_DTYPE_FP8_E4M3 : c->cfg.dtype;
-  const uint64_t es = s.fp8 ? 1 : 2;   // bytes per element (int4: per two codes, counted below in bytes)
-  const uint64_t kH = s.int4 ? (uint64_t)s.H / 2 : (uint64_t)s.H, kI = s.int4 ? (uint64_t)s.I / 2 : (uint64_t)s.I;
-  const uint64_t rH = s.int4 ? kH : (uint64_t)s.H * es, rI = s.int4 ? kI : (uint64_t)s.I * es;   // row strides in bytes
+  const uint64_t es = s.bits < 16 ? 1 : 2;                                          // bytes per map element (encode_map)
+  const uint64_t rH = (uint64_t)s.H * s.bits / 8, rI = (uint64_t)s.I * s.bits / 8;   // bytes per row of K = H / K = I
+  const uint32_t box[3] = {(uint32_t)(64 * s.bits / 8 / es), box_rows, 1};          // one k-row of a 64-wide k-block
   {
-    const uint64_t dims[3] = {kH, (uint64_t)s.I, (uint64_t)a->nslots};
+    const uint64_t dims[3] = {rH / es, (uint64_t)s.I, (uint64_t)a->nslots};
     const uint64_t str[2] = {rH, (uint64_t)a->slot_bytes};
-    int r = encode_map(c, tg, dt, a->base + s.off_gate, 3, dims, str, box);
+    int r = encode_map(c, tg, s.bits, a->base + s.off_gate, 3, dims, str, box);
     if (r) return r;
-    r = encode_map(c, tu, dt, a->base + s.off_up, 3, dims, str, box);
+    r = encode_map(c, tu, s.bits, a->base + s.off_up, 3, dims, str, box);
     if (r) return r;
   }
   {
-    const uint64_t dims[3] = {kI, (uint64_t)s.H, (uint64_t)a->nslots};
+    const uint64_t dims[3] = {rI / es, (uint64_t)s.H, (uint64_t)a->nslots};
     const uint64_t str[2] = {rI, (uint64_t)a->slot_bytes};
-    int r = encode_map(c, td, dt, a->base + s.off_down, 3, dims, str, box);
+    int r = encode_map(c, td, s.bits, a->base + s.off_down, 3, dims, str, box);
     if (r) return r;
   }
   return B2M_OK;
@@ -383,7 +383,7 @@ int build_act_map(b2m_ctx* c, CUtensorMap* tm, void* base, int K, int rows, int 
   const uint64_t dims[2] = {(uint64_t)K, (uint64_t)rows};
   const uint64_t str[1] = {(uint64_t)K * 2};
   const uint32_t box[2] = {64, (uint32_t)nt};
-  return encode_map(c, tm, c->cfg.dtype, base, 2, dims, str, box);
+  return encode_map(c, tm, 16, base, 2, dims, str, box);
 }
 
 int nt_index(int nt) { return nt == 16 ? 0 : nt == 32 ? 1 : nt == 64 ? 2 : nt == 128 ? 3 : 4; }
@@ -766,12 +766,10 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (!cfg || !out) return fail(nullptr, B2M_EINVAL, "null argument");
   if (cfg->struct_size != (int)sizeof(b2m_config))
     return fail(nullptr, B2M_EINVAL, "b2m_config size mismatch (%d vs %d)", cfg->struct_size, (int)sizeof(b2m_config));
-  if (weight_format != B2M_WEIGHTS_MODEL_DTYPE && weight_format != B2M_WEIGHTS_FP8_E4M3_B128 &&
-      weight_format != B2M_WEIGHTS_INT4_G128 && weight_format != B2M_WEIGHTS_INT4_G128_F16)
-    return fail(nullptr, B2M_EINVAL, "unknown weight format %d", weight_format);
-  // (the two int4 formats share the slot layout; their group scales are of the activations' type, bf16 or f16)
-  const bool fp8 = weight_format == B2M_WEIGHTS_FP8_E4M3_B128, int4_f16 = weight_format == B2M_WEIGHTS_INT4_G128_F16,
-             int4 = weight_format == B2M_WEIGHTS_INT4_G128 || int4_f16;
+  const WeightFormat* wf = nullptr;
+  for (const WeightFormat& f : WEIGHT_FORMATS)
+    if (f.id == weight_format) wf = &f;
+  if (!wf) return fail(nullptr, B2M_EINVAL, "unknown weight format %d", weight_format);
   if (cfg->dtype == B2M_DTYPE_FP8_E4M3)
     return fail(nullptr, B2M_EUNSUPPORTED, "dtype %d (fp8): the reference's own torch::matmul has no Float8 kernel; bf16, f16 and f32 experts are supported", cfg->dtype);
   if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16 && cfg->dtype != B2M_DTYPE_F32) return fail(nullptr, B2M_EINVAL, "bad dtype");
@@ -781,34 +779,22 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       cfg->max_tokens < 1)
     return fail(nullptr, B2M_EINVAL, "bad model dimensions");
   ExpertShape shape;
-  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, &shape, fp8 || int4 ? 1 : esize))
+  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, wf->bits ? wf->bits : 8 * (int)esize,
+                  wf->grid_bytes ? wf->grid_bytes(cfg->hidden, cfg->inter) : 0, &shape))
     return fail(nullptr, B2M_EUNSUPPORTED, "expert_type %d is unknown (expert_module.h:13-18 defines 0..5)", cfg->expert_type);
-  if (fp8) {
-    if (cfg->dtype != B2M_DTYPE_BF16)
-      return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights need a bf16 model dtype (activations), got dtype %d", cfg->dtype);
+  if (wf->a_src != AS_BF16) {   // a quantised format: three matrices per expert, decoded inside the tensor-core GEMMs
+    if (cfg->dtype != wf->act_dtype)
+      return fail(nullptr, B2M_EUNSUPPORTED, "%s weights need %s activations (model dtype), got dtype %d", wf->name,
+                  wf->act_dtype == B2M_DTYPE_BF16 ? "bf16" : "f16", cfg->dtype);
     if (cfg->expert_type != B2M_EXPERT_MIXTRAL_MOE_DENSE_ACT_DENSE && cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
-      return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights support Mixtral (4) and DeepSeek (5) experts, got expert_type %d", cfg->expert_type);
-    if (cfg->hidden % f8::BLOCK || cfg->inter % f8::BLOCK)
-      return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights need hidden and inter to be multiples of %d (128x128 scale blocks), got %d / %d",
-                  f8::BLOCK, cfg->hidden, cfg->inter);
+      return fail(nullptr, B2M_EUNSUPPORTED, "%s weights support Mixtral (4) and DeepSeek (5) experts, got expert_type %d",
+                  wf->name, cfg->expert_type);
+    if (cfg->hidden % wf->hi_multiple || cfg->inter % wf->hi_multiple)
+      return fail(nullptr, B2M_EUNSUPPORTED, "%s weights need hidden and inter to be multiples of %d (scale blocks or groups, "
+                  "128-row tiles), got %d / %d", wf->name, wf->hi_multiple, cfg->hidden, cfg->inter);
     if (cfg->gemm_impl == 1)
-      return fail(nullptr, B2M_EUNSUPPORTED, "fp8 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
-    make_fp8_shape(&shape);
-  }
-  if (int4) {
-    if (int4_f16 && cfg->dtype != B2M_DTYPE_F16)
-      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights with fp16 scales need an f16 model dtype (activations), got dtype %d",
-                  cfg->dtype);
-    if (!int4_f16 && cfg->dtype != B2M_DTYPE_BF16)
-      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights need a bf16 model dtype (activations), got dtype %d", cfg->dtype);
-    if (cfg->expert_type != B2M_EXPERT_MIXTRAL_MOE_DENSE_ACT_DENSE && cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
-      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights support Mixtral (4) and DeepSeek (5) experts, got expert_type %d", cfg->expert_type);
-    if (cfg->hidden % i4::GROUP || cfg->inter % i4::GROUP)
-      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights need hidden and inter to be multiples of %d (128-input groups, 128-row tiles), got %d / %d",
-                  i4::GROUP, cfg->hidden, cfg->inter);
-    if (cfg->gemm_impl == 1)
-      return fail(nullptr, B2M_EUNSUPPORTED, "int4 weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)");
-    make_int4_shape(&shape);
+      return fail(nullptr, B2M_EUNSUPPORTED, "%s weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)",
+                  wf->name);
   }
   if (cfg->router < 0 || cfg->router > 5) return fail(nullptr, B2M_EINVAL, "bad router kind");
   if (cfg->router == B2M_ROUTER_QWEN_MOE) {
@@ -847,8 +833,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   b2m_ctx* c = new (std::nothrow) b2m_ctx();
   if (!c) return fail(nullptr, B2M_ENOMEM, "out of host memory");
   c->cfg = *cfg;
-  c->fp8 = fp8;
-  c->int4 = int4;
+  c->wf = wf;
   memset(&c->stats, 0, sizeof c->stats);
 #define CKC(call)                                                                                     \
   do {                                                                                                \
@@ -894,7 +879,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   c->offload = nslots < (long long)L * E;
   CKC(cudaMalloc((void**)&c->arena.base, (size_t)nslots * shape.bytes));
   c->arena.owned = true;
-  for (int m = 0; m < 3 && !fp8 && !int4; ++m) {   // (an fp8 / int4 context has no 12-bit packed copy: pk.slot_bytes stays 0)
+  for (int m = 0; m < 3 && wf->a_src == AS_BF16; ++m) {   // (a quantised context has no 12-bit packed copy: pk.slot_bytes stays 0)
     c->pk.off[m] = c->pk.slot_bytes;
     c->pk.slot_bytes += packed_matrix_bytes((int)pk_matrix_rows(shape, m), (int)pk_matrix_cols(shape, m));
   }
@@ -904,7 +889,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (r) { g_create_error = c->err; b2m_ctx_destroy(c); return r; }
   if (cfg->shared_inter > 0) {
     ExpertShape ss;
-    make_shape(B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, H, cfg->shared_inter, &ss, esize);
+    make_shape(B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, H, cfg->shared_inter, 8 * (int)esize, 0, &ss);
     c->shared_arena.shape = ss;
     c->shared_arena.slot_bytes = ss.bytes;
     c->shared_arena.nslots = L;
@@ -1109,7 +1094,7 @@ int b2m_set_shared_gate(b2m_ctx* c, int layer, const void* dev_w) {
 int b2m_set_input_perm(b2m_ctx* c, int layer, const uint16_t* dev_perm) {
   int r = check_layer(c, layer);
   if (r) return r;
-  if (!c->int4 || c->cfg.dtype != B2M_DTYPE_F16)
+  if (c->wf->id != B2M_WEIGHTS_INT4_G128_F16)
     return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations (act-order GPTQ) need a B2M_WEIGHTS_INT4_G128_F16 "
                 "context");
   c->input_perm[layer] = dev_perm;
@@ -1349,17 +1334,12 @@ static int launch_expert_gemms(b2m_ctx* c, Arena& a, const GemmParams& base, con
     // packed weights (decode-sized tiles of the routed experts); this call's gate/up launch first packs the stale slots it
     // was handed (base.pack_slots), the down launch never packs
     dn.pack_n = 0;
-    if (&a == &c->arena && s.fp8) {
-      up.f8_s0 = a.base + s.sc_gate;
-      up.f8_s1 = a.base + s.sc_up;
-      dn.f8_s0 = dn.f8_s1 = a.base + s.sc_down;
-      up.f8_slot_bytes = dn.f8_slot_bytes = a.slot_bytes;
-    }
-    if (&a == &c->arena && s.int4) {
-      up.i4_g0 = a.base + s.sc_gate;
-      up.i4_g1 = a.base + s.sc_up;
-      dn.i4_g0 = dn.i4_g1 = a.base + s.sc_down;
-      up.i4_slot_bytes = dn.i4_slot_bytes = a.slot_bytes;
+    if (&a == &c->arena && c->wf->a_src != AS_BF16) {   // (shared experts are always in the model dtype)
+      up.a_src = dn.a_src = c->wf->a_src;
+      up.grid0 = a.base + s.grid_gate;
+      up.grid1 = a.base + s.grid_up;
+      dn.grid0 = dn.grid1 = a.base + s.grid_down;
+      up.grid_slot_bytes = dn.grid_slot_bytes = a.slot_bytes;
     }
     if (&a == &c->arena && c->pk.state == 1) {
       up.pk_ok = dn.pk_ok = c->pk.d_ok;
@@ -1897,8 +1877,7 @@ static EpParams ep_base(b2m_ctx* c, int nranks, int rank, int cap) {
 static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (!c) return B2M_EINVAL;
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
-  if (c->fp8) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with fp8 weights");
-  if (c->int4) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with int4 weights");
+  if (c->wf->a_src != AS_BF16) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with %s weights", c->wf->name);
   if (c->cfg.router == B2M_ROUTER_QWEN_MOE) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the qwen_moe router");
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
     return fail(c, B2M_EINVAL, "bad expert-parallel geometry (nranks=%d rank=%d cap=%d E=%d)", nranks, rank, cap, c->cfg.num_experts);

@@ -30,6 +30,12 @@ enum : int {
                          // sigmoid(x[t] . shared_gate_w) in the model dtype (x [T,H], shared_gate_w [H], out [T], 16-bit)
 };
 
+// Where a tensor-core GEMM's A operand (the weight tile) comes from: GemmParams::a_src, the kernels' AS template parameter
+enum : int { AS_BF16 = 0,   // bf16 tile in shared memory, read by the wgmma itself
+             AS_PK12 = 1,   // bf16 tile or 12-bit packed record (weight_pack.cuh), decoded into register fragments
+             AS_FP8 = 2,    // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
+             AS_INT4 = 3 }; // 4-bit code tile + per-128-input scale / zero point (int4_weights.cuh), dequantised likewise
+
 struct GemmParams {
   const int* offsets;   // [E+1] first permuted row of each expert
   const int* slot_of;   // [E]   HBM slot of each expert of this layer (-1: not resident -> skipped)
@@ -94,16 +100,13 @@ struct GemmParams {
   int pack_rows[3], pack_cols[3];
   uint8_t* pack_dst;         // packed arena (pk_slot_bytes per slot)
   int* pack_ok;              // = pk_ok, writable
-  // ---- fp8 weights (fp8_weights.cuh; bf16 activations): non-null = the A maps are uint8 maps over e4m3 matrices and
-  // f8_s0 / f8_s1 are the fp32 block-scale grids [M / 128][K / 128] of A0 / A1 in slot 0, f8_slot_bytes apart
-  const uint8_t* f8_s0;
-  const uint8_t* f8_s1;
-  size_t f8_slot_bytes;
-  // ---- int4 weights (int4_weights.cuh; bf16 or f16 activations): non-null = the A maps are uint8 maps over 4-bit code matrices and
-  // i4_g0 / i4_g1 are the tile-major group grids (one uint32 per row and 128 k) of A0 / A1 in slot 0, i4_slot_bytes apart
-  const uint8_t* i4_g0;
-  const uint8_t* i4_g1;
-  size_t i4_slot_bytes;
+  // ---- quantised weights (AS_FP8, AS_INT4): the A maps are uint8 maps over the quantised matrices, and grid0 / grid1 are
+  // the side grids of A0 / A1 in slot 0, grid_slot_bytes apart: fp32 block scales [M / 128][K / 128] (fp8_weights.cuh) or
+  // tile-major group words, one uint32 per row and 128 k (int4_weights.cuh)
+  const uint8_t* grid0;
+  const uint8_t* grid1;
+  size_t grid_slot_bytes;
+  int a_src;                 // AS_*: how the GEMM reads its A operand (read by the launcher, which picks the kernel)
 };
 
 // packed copy of a rows x cols K-major bf16 matrix (weight_pack.cuh); 0 when its shape does not divide into tiles
@@ -123,7 +126,6 @@ cudaError_t launch_grouped_gemm_simt(int dtype, const void* arena, size_t slot_e
 cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& gate, const CUtensorMap& upm, const CUtensorMap& b_up,
                              const CUtensorMap& down, const CUtensorMap& b_down, const GemmParams& up, const GemmParams& dn,
                              int grid, int up_ctas, int* gbar, cudaStream_t st);
-int gemm_tc_smem_bytes(int nt, bool dual);
 // fp32 experts (dtype int 1): CUDA-core fp32 FMA kernel, f32_path.cu.  Offsets/slot sizes in fp32 elements.
 cudaError_t launch_grouped_gemm_f32(const void* arena, size_t slot_elems, size_t offA0, size_t offA1, const void* B,
                                     int ldb, const GemmParams& p, bool dual, int num_sms, cudaStream_t st);

@@ -38,12 +38,6 @@ constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
 constexpr int MAX_E = 256;
 constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on sm_90; the rest holds barriers and tile tables
 
-// Where a GEMM's A operand (the weight tile) comes from
-enum : int { AS_BF16 = 0,   // bf16 tile in shared memory, read by the wgmma itself
-             AS_PK12 = 1,   // bf16 tile or 12-bit packed record (weight_pack.cuh), decoded into register fragments
-             AS_FP8 = 2,    // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
-             AS_INT4 = 3 }; // 4-bit code tile + per-128-input scale / zero point (int4_weights.cuh), dequantised likewise
-
 template <int NT, bool DUAL, int AS = AS_BF16>
 struct GemmCfg {
   static constexpr int A_BYTES = AS == AS_FP8 ? f8::TILE_BYTES : AS == AS_INT4 ? i4::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
@@ -397,8 +391,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       float sn0 = 0.f, sn1 = 0.f;
       if constexpr (F8) {
         const int kbs = p.K / f8::BLOCK, mt = t.m0 / BLOCK_M, mts = p.M / BLOCK_M;
-        sc0 = reinterpret_cast<const float*>(p.f8_s0 + (size_t)t.slot * p.f8_slot_bytes) + (size_t)mt * kbs;
-        sc1 = DUAL ? reinterpret_cast<const float*>(p.f8_s1 + (size_t)t.slot * p.f8_slot_bytes) +
+        sc0 = reinterpret_cast<const float*>(p.grid0 + (size_t)t.slot * p.grid_slot_bytes) + (size_t)mt * kbs;
+        sc1 = DUAL ? reinterpret_cast<const float*>(p.grid1 + (size_t)t.slot * p.grid_slot_bytes) +
                          (size_t)(p.dual_m && mt + 1 < mts ? mt + 1 : mt) * kbs
                    : sc0;
         sn0 = __ldg(sc0 + t.kb_begin / 2);
@@ -423,8 +417,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       std::conditional_t<I4, I4Groups, NoGroups> grp;
       if constexpr (I4) {
         const int gs = p.K / i4::GROUP, mt = t.m0 / BLOCK_M, mts = p.M / BLOCK_M;
-        grp.w[0] = reinterpret_cast<const uint32_t*>(p.i4_g0 + (size_t)t.slot * p.i4_slot_bytes) + (size_t)mt * gs * BLOCK_M + ra;
-        grp.w[1] = DUAL ? reinterpret_cast<const uint32_t*>(p.i4_g1 + (size_t)t.slot * p.i4_slot_bytes) +
+        grp.w[0] = reinterpret_cast<const uint32_t*>(p.grid0 + (size_t)t.slot * p.grid_slot_bytes) + (size_t)mt * gs * BLOCK_M + ra;
+        grp.w[1] = DUAL ? reinterpret_cast<const uint32_t*>(p.grid1 + (size_t)t.slot * p.grid_slot_bytes) +
                               (size_t)(p.dual_m && mt + 1 < mts ? mt + 1 : mt) * gs * BLOCK_M + ra
                         : grp.w[0];
         grp.load(t.kb_begin);
@@ -763,74 +757,23 @@ cudaError_t launch_fused_ffn(int dtype, int nt, const CUtensorMap& g, const CUte
 
 #endif  // B2M_ENABLE_FUSED_FFN
 
-template <int DT>
-static cudaError_t dispatch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
-                               const GemmParams& p, int grid, cudaStream_t st) {
-  // int4 weights (bf16 or f16 scales and activations): every tile width the plan of the DT engine picks, same plan (the
-  // caller's p)
-  if (p.i4_g0) {
-#define B2M_ICASE(N)                                                                \
-  case N:                                                                           \
-    return dual ? launch_tc<N, true, DT, 1, AS_INT4>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
-    switch (nt) {
-      B2M_ICASE(16)
-      B2M_ICASE(32)
-      B2M_ICASE(64)
-      B2M_ICASE(128)
-      case 256:
-        return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_INT4>(a0, a1, b, p, grid, st);
-      default:
-        return cudaErrorInvalidValue;
-    }
-#undef B2M_ICASE
-  }
-  // fp8 weights: every tile width the bf16 plan picks, same plan (the caller's p)
-  if constexpr (DT == DT_BF16) {
-    if (p.f8_s0) {
-#define B2M_FCASE(N)                                                                \
-  case N:                                                                           \
-    return dual ? launch_tc<N, true, DT, 1, AS_FP8>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_FP8>(a0, a1, b, p, grid, st);
-      switch (nt) {
-        B2M_FCASE(16)
-        B2M_FCASE(32)
-        B2M_FCASE(64)
-        B2M_FCASE(128)
-        case 256:
-          return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS_FP8>(a0, a1, b, p, grid, st);
-        default:
-          return cudaErrorInvalidValue;
-      }
-#undef B2M_FCASE
-    }
-  }
-  // packed weights: decode-sized tiles only (at prefill the GEMM is tensor-bound and keeps the shared-memory A operand)
-  if constexpr (DT == DT_BF16) {
-    if (p.pk_ok && nt <= 64 && !p.dual_m && p.m_rows == 0 && p.ep_rows == 0) {
-#define B2M_PCASE(N)                                                                \
-  case N:                                                                           \
-    return dual ? launch_tc<N, true, DT, 1, AS_PK12>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT, 1, AS_PK12>(a0, a1, b, p, grid, st);
-      switch (nt) {
-        B2M_PCASE(16)
-        B2M_PCASE(32)
-        B2M_PCASE(64)
-      }
-#undef B2M_PCASE
-    }
-  }
-#define B2M_CASE(N)                                                                 \
-  case N:                                                                           \
-    return dual ? launch_tc<N, true, DT>(a0, a1, b, p, grid, st) : launch_tc<N, false, DT>(a0, a1, b, p, grid, st);
+// one kernel per token-tile width for the A source AS (256-token tiles: single projections only, GemmCfg; packed records:
+// decode-sized tiles only)
+template <int DT, int AS>
+static cudaError_t launch_nt(int nt, bool dual, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b,
+                             const GemmParams& p, int grid, cudaStream_t st) {
   switch (nt) {
-    B2M_CASE(16)
-    B2M_CASE(32)
-    B2M_CASE(64)
-    B2M_CASE(128)
-    case 256:   // single projections only (GemmCfg)
-      return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT>(a0, a1, b, p, grid, st);
-    default:
-      return cudaErrorInvalidValue;
+    case 16: return dual ? launch_tc<16, true, DT, 1, AS>(a0, a1, b, p, grid, st) : launch_tc<16, false, DT, 1, AS>(a0, a1, b, p, grid, st);
+    case 32: return dual ? launch_tc<32, true, DT, 1, AS>(a0, a1, b, p, grid, st) : launch_tc<32, false, DT, 1, AS>(a0, a1, b, p, grid, st);
+    case 64: return dual ? launch_tc<64, true, DT, 1, AS>(a0, a1, b, p, grid, st) : launch_tc<64, false, DT, 1, AS>(a0, a1, b, p, grid, st);
   }
-#undef B2M_CASE
+  if constexpr (AS != AS_PK12) {
+    switch (nt) {
+      case 128: return dual ? launch_tc<128, true, DT, 1, AS>(a0, a1, b, p, grid, st) : launch_tc<128, false, DT, 1, AS>(a0, a1, b, p, grid, st);
+      case 256: return dual ? cudaErrorInvalidValue : launch_tc<256, false, DT, 1, AS>(a0, a1, b, p, grid, st);
+    }
+  }
+  return cudaErrorInvalidValue;
 }
 
 #ifdef B2M_ENABLE_MC2
@@ -984,8 +927,21 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
     q.pdl_edge = 0;
     return launch_grouped_gemm_tc(dtype, nt, dual, a0, a1, b, q, grid, st);
   }
-  if (dtype == DT_BF16) return dispatch_nt<DT_BF16>(nt, dual, a0, a1, b, p, grid, st);
-  if (dtype == DT_F16 && !p.f8_s0) return dispatch_nt<DT_F16>(nt, dual, a0, a1, b, p, grid, st);   // (fp8 weights: bf16 only)
+  // packed weights: decode-sized tiles only (at prefill the GEMM is tensor-bound and keeps the shared-memory A operand)
+  const bool pk = p.pk_ok && nt <= 64 && !p.dual_m && p.m_rows == 0 && p.ep_rows == 0;
+  if (dtype == DT_BF16) {
+    switch (p.a_src) {
+      case AS_BF16: return pk ? launch_nt<DT_BF16, AS_PK12>(nt, dual, a0, a1, b, p, grid, st)
+                              : launch_nt<DT_BF16, AS_BF16>(nt, dual, a0, a1, b, p, grid, st);
+      case AS_FP8: return launch_nt<DT_BF16, AS_FP8>(nt, dual, a0, a1, b, p, grid, st);
+      case AS_INT4: return launch_nt<DT_BF16, AS_INT4>(nt, dual, a0, a1, b, p, grid, st);
+    }
+  } else if (dtype == DT_F16) {   // (no packed copy, no fp8 weights)
+    switch (p.a_src) {
+      case AS_BF16: return launch_nt<DT_F16, AS_BF16>(nt, dual, a0, a1, b, p, grid, st);
+      case AS_INT4: return launch_nt<DT_F16, AS_INT4>(nt, dual, a0, a1, b, p, grid, st);
+    }
+  }
   return cudaErrorInvalidValue;
 }
 
@@ -1001,17 +957,6 @@ cudaError_t launch_grouped_gemm_simt(int dtype, const void* arena, size_t slot_e
   else
     return cudaErrorInvalidValue;
   return cudaGetLastError();
-}
-
-int gemm_tc_smem_bytes(int nt, bool dual) {
-  switch (nt) {
-    case 16: return dual ? GemmCfg<16, true>::SMEM_BYTES : GemmCfg<16, false>::SMEM_BYTES;
-    case 32: return dual ? GemmCfg<32, true>::SMEM_BYTES : GemmCfg<32, false>::SMEM_BYTES;
-    case 64: return dual ? GemmCfg<64, true>::SMEM_BYTES : GemmCfg<64, false>::SMEM_BYTES;
-    case 128: return dual ? GemmCfg<128, true>::SMEM_BYTES : GemmCfg<128, false>::SMEM_BYTES;
-    case 256: return dual ? -1 : GemmCfg<256, false>::SMEM_BYTES;
-  }
-  return -1;
 }
 
 }  // namespace b2m

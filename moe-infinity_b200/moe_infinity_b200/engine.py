@@ -114,15 +114,7 @@ class MoEEngine:
         self._perms: Dict[int, torch.Tensor] = {}
         self._shared_gates: Dict[int, torch.Tensor] = {}
         es = self.esize = 4 if dtype == torch.float32 else 2   # fp32 experts (dtype int 1) run on the CUDA-core fp32 path
-        if expert_type in (L.EXPERT_NLLB, L.EXPERT_FSGPT):     # fc1 | fc1_bias | fc2 | fc2_bias (expert_module.cpp:70-77)
-            self.expert_bytes = 2 * hidden * inter * es + (inter + hidden) * es
-        else:
-            nmat = 2 if expert_type == L.EXPERT_SWITCH else 3
-            self.expert_bytes = nmat * hidden * inter * es
-        if self.fp8:
-            self.expert_bytes = F8.expert_blob_bytes(hidden, inter)
-        if self.int4:
-            self.expert_bytes = I4.expert_blob_bytes(hidden, inter)
+        self.expert_bytes = self.stats()["slot_bytes"]          # one expert blob in the context's weight format
         self.shared_bytes = 3 * hidden * shared_inter * es
 
     # ------------------------------------------------------------------ lifecycle
