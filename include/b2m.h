@@ -92,6 +92,27 @@ extern "C" {
  * With B2M_NUMERICS_FP32: acc += w * y, then acc += g * s, rounded once.  A forward or combine of a layer with shared experts
  * and no gate returns B2M_ESTATE.  The expert-parallel entry points return B2M_EUNSUPPORTED on such a context. */
 #define B2M_ROUTER_QWEN_MOE 5
+/* Llama 4 router (transformers Llama4Router + Llama4TextMoe).  Per token:
+ *   1. logits in the model dtype                           (F.linear in bf16/f16: the fp32 dot is rounded to the model dtype)
+ *   2. top_k experts by the logits themselves              ties go to the lowest index (not by sigmoid values: two logits
+ *                                                          can share one fp32 sigmoid)
+ *   3. w = round(sigmoid(logit)) for each chosen expert    fp32 sigmoid (PyTorch's CUDA formula), rounded to the model dtype
+ *                                                          and stored as fp32 in B2M_WS_TOPK_W; B2M_WS_SCORES holds the
+ *                                                          unrounded fp32 sigmoid of every logit
+ *   4. the input row of (t, e) is round(x[t] * w)          elementwise: the routing weight scales the expert's INPUT, so
+ *                                                          B2M_WS_XP rows hold scaled activations
+ * Accepted by b2m_ctx_create_ex (B2M_EINVAL with a message naming llama4 otherwise) only with expert_type
+ * B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE (gate|up|down), dtype bf16 or f16, n_group = topk_group = 1,
+ * routed_scaling_factor = 1.0, norm_topk_prob = 0 and shared_inter > 0 (every Llama 4 MoE layer has its ungated shared
+ * expert); every weight format works with its own restrictions.  gate_dtype is normally the model dtype; B2M_WS_LOGITS
+ * holds model-dtype logits.
+ * Combine (Llama4TextMoe.forward: routed_out.reshape(k, T, H).sum(0), then shared_expert(x).add_), per element:
+ *   r = round(sum of round(y_e) over the chosen experts)   fp32 sum in ascending expert id, rounded ONCE
+ *   out = round(r + round(s))                               s: fp32 shared-expert output (B2M_WS_Y_SHARED)
+ * With B2M_NUMERICS_FP32: out = round(sum of y_e + s).  The weights are not applied after the experts.
+ * router_in_kind 2 (scores given), b2m_set_input_perm and the expert-parallel entry points return B2M_EUNSUPPORTED on
+ * such a context.  b2m_route_from_mask keeps weight 1: its gathered rows are the unscaled inputs. */
+#define B2M_ROUTER_LLAMA4 6
 
 /* numerics of epilogue + combine */
 #define B2M_NUMERICS_REFERENCE 0 /* replay the reference's per-ATen-op rounding to the model dtype */
@@ -298,7 +319,8 @@ int b2m_moe_forward(b2m_ctx* ctx, int layer, const void* x, const void* router_i
 int b2m_route(b2m_ctx* ctx, int layer, const void* x, const void* router_in, int router_in_kind, int router_in_dtype,
               int T, int seq_len, void* stream);
 /* replaces ExpertDispatcher::SetInputs + per-expert boolean-mask gather (expert_dispatcher.h:66-70,
- * expert_dispatcher.cpp:274-285): routing taken from a dense uint8 mask [T,E] */
+ * expert_dispatcher.cpp:274-285): routing taken from a dense uint8 mask [T,E].  Every weight is 1 (B2M_ROUTER_LLAMA4:
+ * the gathered rows are the unscaled inputs) */
 int b2m_route_from_mask(b2m_ctx* ctx, int layer, const void* x, const uint8_t* mask, int T, void* stream);
 /* replaces EnqueueExpert*n + GPUFetchFunc/GPUExecFunc (expert_dispatcher.cpp:111-395) for the routed tokens
  * currently in the workspace: residency (on demand fetch + eviction) and both grouped GEMMs */
@@ -322,11 +344,12 @@ int b2m_check_errors(b2m_ctx* ctx, void* stream);
 #define B2M_WS_PERM_TOKEN 3 /* int32 [T*k]  source token of each permuted row */
 #define B2M_WS_COUNTS 4     /* int32 [E] */
 #define B2M_WS_OFFSETS 5    /* int32 [E+1] */
-#define B2M_WS_XP 6         /* dtype [T*k,H] */
+#define B2M_WS_XP 6         /* dtype [T*k,H] (B2M_ROUTER_LLAMA4: round(x[t] * w) per row) */
 #define B2M_WS_HMID 7       /* dtype [T*k,I] */
 #define B2M_WS_Y 8          /* fp32  [T*k,H] */
-#define B2M_WS_SCORES 9     /* fp32  [T,E] softmax probabilities (B2M_ROUTER_DEEPSEEK_V3: unbiased sigmoid scores) */
-#define B2M_WS_LOGITS 10    /* router logits computed by the fused gate: model dtype (Mixtral, Qwen) or fp32 */
+#define B2M_WS_SCORES 9     /* fp32  [T,E] softmax probabilities (B2M_ROUTER_DEEPSEEK_V3: unbiased sigmoid scores;
+                               B2M_ROUTER_LLAMA4: sigmoid of every logit, unrounded) */
+#define B2M_WS_LOGITS 10    /* router logits computed by the fused gate: model dtype (Mixtral, Qwen, Llama 4) or fp32 */
 #define B2M_WS_SHARED_GATE 11 /* dtype [T]   B2M_ROUTER_QWEN_MOE with shared experts: sigmoid(shared_expert_gate(x)), rounded
                                  (B2M_ESTATE on other contexts) */
 #define B2M_WS_Y_SHARED 12  /* fp32  [T,H] shared-expert output (B2M_ESTATE on a context without shared experts) */

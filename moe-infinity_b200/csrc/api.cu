@@ -796,7 +796,26 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       return fail(nullptr, B2M_EUNSUPPORTED, "%s weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)",
                   wf->name);
   }
-  if (cfg->router < 0 || cfg->router > 5) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router < 0 || cfg->router > 6) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (cfg->router == B2M_ROUTER_LLAMA4) {
+    if (cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: experts are gate|up|down (expert_type %d), got expert_type %d",
+                  B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, cfg->expert_type);
+    if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: the model dtype must be bf16 or f16, got dtype %d", cfg->dtype);
+    if (cfg->n_group != 1 || cfg->topk_group != 1)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: no group-limited routing (n_group=%d, topk_group=%d must be 1)",
+                  cfg->n_group, cfg->topk_group);
+    if (cfg->routed_scaling_factor != 1.0f)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: weights are not scaled (routed_scaling_factor=%g must be 1.0)",
+                  (double)cfg->routed_scaling_factor);
+    if (cfg->norm_topk_prob)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: weights are not normalised (norm_topk_prob=%d must be 0)",
+                  cfg->norm_topk_prob);
+    if (cfg->shared_inter <= 0)
+      return fail(nullptr, B2M_EINVAL, "llama4 router: every Llama 4 MoE layer has a shared expert (shared_inter=%d must be > 0)",
+                  cfg->shared_inter);
+  }
   if (cfg->router == B2M_ROUTER_QWEN_MOE) {
     if (cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
       return fail(nullptr, B2M_EINVAL, "qwen_moe router: experts are gate|up|down (expert_type %d), got expert_type %d",
@@ -1094,6 +1113,8 @@ int b2m_set_shared_gate(b2m_ctx* c, int layer, const void* dev_w) {
 int b2m_set_input_perm(b2m_ctx* c, int layer, const uint16_t* dev_perm) {
   int r = check_layer(c, layer);
   if (r) return r;
+  if (c->cfg.router == B2M_ROUTER_LLAMA4)
+    return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations are not available with the llama4 router");
   if (c->wf->id != B2M_WEIGHTS_INT4_G128_F16)
     return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations (act-order GPTQ) need a B2M_WEIGHTS_INT4_G128_F16 "
                 "context");
@@ -1216,7 +1237,10 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
     p.logits_dtype = in_dtype;
     p.logits_are_scores = (kind == 2);
     if (kind == 2 && in_dtype != B2M_DTYPE_F32) return fail(c, B2M_EINVAL, "scores must be fp32");
+    if (kind == 2 && c->cfg.router == B2M_ROUTER_LLAMA4)
+      return fail(c, B2M_EUNSUPPORTED, "llama4 router: takes logits (router_in_kind 0 or 1), not scores: it ranks the logits");
   }
+  p.scale_rows = c->cfg.router == B2M_ROUTER_LLAMA4;   // the routing weight scales the expert's input row
   if (c->cfg.router == B2M_ROUTER_SWITCH_TOP1 && (p.seq_len <= 0 || T % p.seq_len))
     return fail(c, B2M_EINVAL, "T=%d is not a multiple of seq_len=%d", T, p.seq_len);
   if (c->cfg.router == B2M_ROUTER_DEEPSEEK_V3 && !p.gate_bias)
@@ -1678,7 +1702,9 @@ static int combine_impl(b2m_ctx* c, int layer, const void* x, int T, void* out, 
   if (f.router == B2M_ROUTER_SWITCH_TOP1) p.mode = COMBINE_SWITCH;
   else if (f.numerics == B2M_NUMERICS_FP32) p.mode = COMBINE_FP32;
   else if (f.router == B2M_ROUTER_QWEN_MOE) p.mode = COMBINE_QWEN;
+  else if (f.router == B2M_ROUTER_LLAMA4) p.mode = COMBINE_LLAMA4;
   else p.mode = f.router == B2M_ROUTER_MIXTRAL ? COMBINE_MIXTRAL : COMBINE_DEEPSEEK;
+  p.unweighted = f.router == B2M_ROUTER_LLAMA4;   // the weights scaled the expert inputs (COMBINE_LLAMA4 or COMBINE_FP32)
   if (f.shared_inter > 0) {
     if (c->shared_in_flight) {
       // launched by b2m_moe_forward on the side stream at the start of the call: join it
@@ -1707,6 +1733,8 @@ int b2m_moe_forward(b2m_ctx* c, int layer, const void* x, const void* router_in,
                     int seq_len, void* out, void* stream) {
   int r = check_layer(c, layer);
   if (r) return r;
+  if (kind == 2 && c->cfg.router == B2M_ROUTER_LLAMA4)   // refused before the shared expert is launched
+    return fail(c, B2M_EUNSUPPORTED, "llama4 router: takes logits (router_in_kind 0 or 1), not scores: it ranks the logits");
   if (c->cfg.shared_inter > 0 && T > 0 && T <= c->cap_T && x) {
     // the shared experts (deepseek.py:133-136) depend on x only: fork them onto a side stream so that their two GEMM
     // launches overlap the gate / top-k / permute kernels of the routed path; b2m_combine joins
@@ -1879,6 +1907,7 @@ static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
   if (c->wf->a_src != AS_BF16) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with %s weights", c->wf->name);
   if (c->cfg.router == B2M_ROUTER_QWEN_MOE) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the qwen_moe router");
+  if (c->cfg.router == B2M_ROUTER_LLAMA4) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the llama4 router");
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
     return fail(c, B2M_EINVAL, "bad expert-parallel geometry (nranks=%d rank=%d cap=%d E=%d)", nranks, rank, cap, c->cfg.num_experts);
   if ((long long)nranks * cap > c->cap_R)

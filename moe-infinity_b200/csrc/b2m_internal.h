@@ -18,6 +18,7 @@ enum : int {
   ROUTER_SWITCH_TOP1 = 3,      // HF 4.x SwitchTransformersTop1Router (switch_transformers.py:76)
   ROUTER_DEEPSEEK_V3 = 4,      // modeling_deepseek_v3/modeling_deepseek.py:466-527 (sigmoid, noaux_tc)
   ROUTER_QWEN_MOE = 5,         // transformers Qwen2MoeTopKRouter / Qwen3MoeTopKRouter (model-dtype logits, fp32 weights)
+  ROUTER_LLAMA4 = 6,           // transformers Llama4Router (top-k of model-dtype logits, rounded sigmoid weights scale the inputs)
 };
 // combine kinds (which reference combine loop is restated)
 enum : int {
@@ -28,6 +29,7 @@ enum : int {
   COMBINE_QWEN = 4,      // Qwen2MoeExperts + Qwen2MoeSparseMoeBlock: product and += rounded, fp32 weights; gated shared expert
   COMBINE_QWEN_GATE = 5, // the first phase of a Qwen2 combine, launched ahead of it on the shared-expert stream: out[t] =
                          // sigmoid(x[t] . shared_gate_w) in the model dtype (x [T,H], shared_gate_w [H], out [T], 16-bit)
+  COMBINE_LLAMA4 = 6,    // Llama4TextMoe: unweighted fp32 sum of the rounded expert outputs, rounded once, + rounded shared
 };
 
 // Where a tensor-core GEMM's A operand (the weight tile) comes from: GemmParams::a_src, the kernels' AS template parameter
@@ -217,6 +219,7 @@ struct RouteParams {
   int ep_dispatch;           // 1 (T <= 256 only): gathered rows go straight to the owning ranks' buffers (ep)
   EpParams ep;
   unsigned long long* tl;    // optional timeline slots: [0] gate/top-k start, [1] its end, [2] permute start, [3] permute end
+  int scale_rows;            // Llama 4: the gathered row of pair i is round(x[t] * topk_w[i]) (written by this routing call)
 };
 cudaError_t launch_route(const RouteParams& p, cudaStream_t st);
 // look-ahead: top-k of the NEXT layer's router (p.gate_w = its weight; DeepSeek-V3: p.gate_bias = its bias) on this layer's
@@ -241,6 +244,7 @@ struct CombineParams {
   unsigned long long* tl;  // optional timeline slots: [0] start, [1] owners' flags seen, [2] end
   const uint16_t* shared_gate;  // Qwen2-MoE: [T] model-dtype sigmoid(shared_expert_gate(x)) scaling y_shared (COMBINE_QWEN_GATE)
   const void* shared_gate_w;    // COMBINE_QWEN_GATE: the layer's [H] shared_expert_gate.weight (model dtype)
+  int unweighted;               // Llama 4 (COMBINE_LLAMA4, or COMBINE_FP32): expert outputs summed without weights, + y_shared
 };
 cudaError_t launch_combine(const CombineParams& p, cudaStream_t st);
 cudaError_t launch_combine_f32(const CombineParams& p, cudaStream_t st);

@@ -32,9 +32,13 @@ __device__ __forceinline__ float load_as_float(const void* p, size_t i, int dt) 
 // bytes of one hidden row of the model dtype (fp32 models: 4-byte elements; rows stay multiples of 16 B since H % 8 == 0)
 __device__ __forceinline__ size_t row_bytes(const RouteParams& p) { return (size_t)p.H * (p.dtype == DT_F32 ? 4 : 2); }
 // Routers whose gate is an nn.Linear in the model dtype: their logits are rounded to the model dtype before the softmax
-// (Mixtral, mixtral.py:46; Qwen2-MoE / Qwen3-MoE, modeling_qwen2_moe.py Qwen2MoeTopKRouter).  The others take fp32 logits.
+// (Mixtral, mixtral.py:46; Qwen2-MoE / Qwen3-MoE, modeling_qwen2_moe.py Qwen2MoeTopKRouter; Llama 4, Llama4Router, which
+// ranks those logits directly).  The others take fp32 logits.  Written as two compares (the router kinds from
+// ROUTER_QWEN_MOE on all take model-dtype logits; b2m_ctx_create_ex admits none above ROUTER_LLAMA4), so that the unrolled
+// gate loops of the other routers compile to the code they had before Llama 4.
+static_assert(ROUTER_LLAMA4 == ROUTER_QWEN_MOE + 1, "logits_in_model_dtype: every router from ROUTER_QWEN_MOE on has model-dtype logits");
 __host__ __device__ __forceinline__ bool logits_in_model_dtype(int router) {
-  return router == ROUTER_MIXTRAL || router == ROUTER_QWEN_MOE;
+  return router == ROUTER_MIXTRAL || router >= ROUTER_QWEN_MOE;
 }
 __device__ __forceinline__ float round_to(float f, int dt) {
   if (dt == DT_BF16) return round_dt<DT_BF16>(f);
@@ -388,6 +392,14 @@ __device__ __forceinline__ void route_token_v3(const RouteParams& p, int t, cons
   __syncwarp();
 }
 
+// Llama 4 pieces of K1, kept out of line so that the other routers' code around them is not rearranged (the routing
+// kernels are instruction-cache cold every launch): the fp32 sigmoid of every logit (B2M_WS_SCORES, one warp, logits in
+// shared memory) and the weight of a chosen logit, round(sigmoid(l)) in the model dtype (Llama4Router).
+__device__ __noinline__ void llama4_scores(const float* s_in, float* scores_row, int E) {
+  for (int e = threadIdx.x & 31; e < E; e += 32) scores_row[e] = sigmoid_ref(s_in[e]);
+}
+__device__ __noinline__ float llama4_weight(float logit, int dtype) { return round_to(sigmoid_ref(logit), dtype); }
+
 // --------------------------------------------------------------------------------------
 // K1: softmax + top-k (+renorm) for one token (one warp, lane owns experts lane, lane+32, ...)
 // --------------------------------------------------------------------------------------
@@ -408,7 +420,8 @@ __device__ void route_token_warp(const RouteParams& p, int t, const float* s_in 
     v[i] = e < E ? s_in[e] : -INFINITY;
     m = fmaxf(m, v[i]);
   }
-  if (!in_are_scores) {
+  // Llama 4 selects on the logits themselves (Llama4Router: torch.topk(router_logits)), so there is no softmax
+  if (!in_are_scores && p.router != ROUTER_LLAMA4) {
     m = warp_max(m);
     float z = 0.f;
 #pragma unroll
@@ -421,7 +434,9 @@ __device__ void route_token_warp(const RouteParams& p, int t, const float* s_in 
 #pragma unroll
     for (int i = 0; i < MAX_PL; ++i) v[i] = __fdiv_rn(v[i], z);
   }
-  if (p.scores) {
+  if (p.scores && p.router == ROUTER_LLAMA4) {
+    llama4_scores(s_in, p.scores + (size_t)t * E, E);
+  } else if (p.scores) {
 #pragma unroll
     for (int i = 0; i < MAX_PL; ++i) {
       const int e = lane + 32 * i;
@@ -495,6 +510,9 @@ __device__ void route_token_warp(const RouteParams& p, int t, const float* s_in 
     } else if (p.router == ROUTER_QWEN_MOE) {
       // Qwen2MoeTopKRouter: fp32 weights, divided by their sum (selection order) for every k, no epsilon, no scaling
       w = p.norm_topk_prob ? __fdiv_rn(sv, denom) : sv;
+    } else if (p.router == ROUTER_LLAMA4) {
+      // Llama4Router: sigmoid(router_scores.float()).to(model dtype) of the chosen logit; it scales the expert's input rows
+      w = llama4_weight(sv, p.dtype);
     } else if (p.k > 1 && p.norm_topk_prob) {
       w = __fdiv_rn(sv, __fadd_rn(denom, 1e-20f));                        // modeling_deepseek.py:508-510
     } else {
@@ -629,17 +647,39 @@ __device__ __noinline__ void gather_row_perm(const uint16_t* __restrict__ src, c
   if (bad && err_flag) atomicOr(err_flag, 2);
 }
 
+// Llama 4 gather of one 16-bit row scaled by its routing weight: dst[c] = round(x[c] * w) (the product of two 16-bit
+// values is exact in fp32, so one __fmul_rn and one rounding to the model dtype), 16-byte loads and stores; threads tid,
+// tid + nthr, ... of the caller share the row.  Not inlined, for the same reason as gather_row_perm.
+__device__ __noinline__ void scale_row(const uint4* __restrict__ src, uint4* __restrict__ dst, int nvec, float w, int dtype,
+                                       int tid, int nthr) {
+  for (int v = tid; v < nvec; v += nthr) {
+    float f[8];
+    unpack8(src[v], dtype, f);
+    uint4 o;
+    uint16_t* os = reinterpret_cast<uint16_t*>(&o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      os[j] = dtype == DT_BF16 ? Half16<DT_BF16>::from_f(__fmul_rn(f[j], w)) : Half16<DT_F16>::from_f(__fmul_rn(f[j], w));
+    dst[v] = o;
+  }
+}
+
 // Copy one activation row x[t] -> dst with 16-byte vectors, NTHR threads (a warp or the whole CTA; `tid` = this thread's
 // index among them).  e = the expert of the row: a layer with an input permutation gathers column c from x[t][perm[e][c]]
-// instead (gather_row_perm; 16-bit models only).
+// instead (gather_row_perm; 16-bit models only).  pair = the row's (token, choice) index t * k + j: a Llama 4 routing call
+// (p.scale_rows) scales the row by topk_w[pair] (scale_row).
 template <int NTHR>
-__device__ __forceinline__ void copy_row(const RouteParams& p, int t, int e, void* dst_row, int tid) {
+__device__ __forceinline__ void copy_row(const RouteParams& p, int t, int e, int pair, void* dst_row, int tid) {
   const size_t rb = row_bytes(p);
   const int vec_per_row = (int)(rb / 16);   // uint4 = 8 x 16-bit (4 x fp32)
   const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + (size_t)t * rb);
   uint4* dst = reinterpret_cast<uint4*>(dst_row);
   if (p.input_perm) {
     gather_row_perm(reinterpret_cast<const uint16_t*>(src), p.input_perm + (size_t)e * p.H, dst, p.H, tid, NTHR, p.err_flag);
+    return;
+  }
+  if (p.scale_rows) {
+    scale_row(src, dst, vec_per_row, p.topk_w[pair], p.dtype, tid, NTHR);
     return;
   }
   int v = tid;
@@ -662,7 +702,7 @@ __device__ void copy_rows_block(const RouteParams& p, int t0, int npairs, const 
     const int t = t0 + i / p.k;
     if (row < 0 || t >= p.T) continue;
     const int e = p.input_perm ? p.topk_idx[(size_t)t0 * p.k + i] : 0;
-    copy_row<32>(p, t, e, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, lane);
+    copy_row<32>(p, t, e, t0 * p.k + i, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, lane);
   }
 }
 
@@ -982,7 +1022,7 @@ __global__ void __launch_bounds__(RT_THREADS) permute_small_kernel(const RoutePa
       const int row = p.row_of[i];
       if (row < 0) continue;
       const int e = p.input_perm ? p.topk_idx[i] : 0;
-      copy_row<RT_THREADS>(p, i / p.k, e, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, threadIdx.x);
+      copy_row<RT_THREADS>(p, i / p.k, e, i, reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb, threadIdx.x);
     }
     if (p.y_zero) {
       float4* z = reinterpret_cast<float4*>(p.y_zero);
@@ -1090,7 +1130,7 @@ __global__ void __launch_bounds__(RT_THREADS) permute_small_kernel(const RoutePa
     } else {
       dst = reinterpret_cast<uint8_t*>(p.xp) + (size_t)row * rb;
     }
-    copy_row<RT_THREADS>(p, t, s_idx[i], dst, threadIdx.x);
+    copy_row<RT_THREADS>(p, t, s_idx[i], i, dst, threadIdx.x);
   }
   if (p.ep_dispatch && p.ep.p2p) p2p_signal(p.ep, 0);
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 3);
@@ -1406,6 +1446,83 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
 }
 
+// --------------------------------------------------------------------------------------
+// Llama 4 combine (Llama4TextMoe.forward): the routing weights already scaled the expert inputs, so the expert outputs are
+// summed without weights -- routed_out.reshape(k, T, H).sum(dim=0) on the model dtype accumulates round(y) in fp32 and
+// rounds once -- and out = shared_expert(x).add_(that sum): round(r + round(s)).  COMBINE_FP32: round(sum of y + s).
+// Experts in ascending id, as in the dense HF sum (its unselected experts add exact zeros).  A kernel of its own, so the
+// instantiations of combine_kernel compile exactly the code they had before this mode existed.
+// --------------------------------------------------------------------------------------
+template <int DT>
+__global__ void __launch_bounds__(CB_THREADS) combine_llama4_kernel(const CombineParams p) {
+  const int t = blockIdx.x;
+  const int lane = threadIdx.x & 31;
+  const int k = p.k;
+  pdl_launch();
+  pdl_wait();
+  if (p.tl && threadIdx.x == 0) tl_min(p.tl);
+  int my_e = 0x7fffffff, my_row = -1;
+  if (lane < k) {
+    my_e = p.topk_idx[(size_t)t * k + lane];
+    my_row = p.row_of[(size_t)t * k + lane];
+    if (my_e < 0 || my_row < 0) { my_e = 0x7ffffff0 + lane; my_row = -1; }
+  }
+  int rank = 0;
+  for (int j = 0; j < k; ++j) rank += (__shfl_sync(0xffffffffu, my_e, j) < my_e) ? 1 : 0;
+  int rows[MAX_K];
+#pragma unroll
+  for (int r = 0; r < MAX_K; ++r) {
+    rows[r] = -1;
+    if (r < k) {
+      const uint32_t who = __ballot_sync(0xffffffffu, lane < k && rank == r);
+      rows[r] = __shfl_sync(0xffffffffu, my_row, __ffs(who) - 1);
+    }
+  }
+  const bool fp32 = p.mode == COMBINE_FP32;
+  const int H = p.H;
+  for (int h = (blockIdx.y * CB_THREADS + threadIdx.x) * 8; h < H; h += gridDim.y * CB_THREADS * 8) {
+    float acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+    // four expert rows in flight at a time (invalid rows read row 0 and are ignored), as in combine_kernel
+#pragma unroll
+    for (int r0 = 0; r0 < MAX_K; r0 += 4) {
+      if (r0 >= k) break;
+      float yk[4][8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = r0 + q;
+        if (r < k) {
+          const float4* src = reinterpret_cast<const float4*>(p.y + (size_t)(rows[r] >= 0 ? rows[r] : 0) * H + h);
+          const float4 a = src[0], b = src[1];
+          yk[q][0] = a.x; yk[q][1] = a.y; yk[q][2] = a.z; yk[q][3] = a.w;
+          yk[q][4] = b.x; yk[q][5] = b.y; yk[q][6] = b.z; yk[q][7] = b.w;
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = r0 + q;
+        if (r < k && rows[r] >= 0) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) acc[i] = __fadd_rn(acc[i], fp32 ? yk[q][i] : round_dt<DT>(yk[q][i]));
+        }
+      }
+    }
+    const float4* src = reinterpret_cast<const float4*>(p.y_shared + (size_t)t * H + h);
+    const float4 a = src[0], b = src[1];
+    const float s[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint4 o;
+    uint16_t* os = reinterpret_cast<uint16_t*>(&o);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float v = fp32 ? __fadd_rn(acc[i], s[i]) : __fadd_rn(round_dt<DT>(acc[i]), round_dt<DT>(s[i]));
+      os[i] = Half16<DT>::from_f(v);
+    }
+    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + (size_t)t * H + h) = o;
+  }
+  if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
+}
+
 static cudaError_t launch_shared_gate(const CombineParams& p, cudaStream_t st);
 
 cudaError_t launch_combine(const CombineParams& p, cudaStream_t st) {
@@ -1415,6 +1532,13 @@ cudaError_t launch_combine(const CombineParams& p, cudaStream_t st) {
   int gy = (p.H + CB_THREADS * 8 - 1) / (CB_THREADS * 8);
   dim3 grid(p.T, gy);
   if (p.dtype == DT_F32) return launch_combine_f32(p, st);
+  if (p.unweighted || p.mode == COMBINE_LLAMA4) {
+    if (!p.unweighted || (p.mode != COMBINE_LLAMA4 && p.mode != COMBINE_FP32) || !p.y_shared || p.ep_collect || p.shared_gate)
+      return cudaErrorInvalidValue;
+    if (p.dtype == DT_BF16) return launch_cluster(combine_llama4_kernel<DT_BF16>, grid, dim3(CB_THREADS), 0, st, 1, false, p);
+    if (p.dtype == DT_F16) return launch_cluster(combine_llama4_kernel<DT_F16>, grid, dim3(CB_THREADS), 0, st, 1, false, p);
+    return cudaErrorInvalidValue;
+  }
   const bool early = p.ep_collect && p.ep.direct && p.ep_early;
   const bool qwen = p.mode == COMBINE_QWEN || p.shared_gate;
   if (qwen && (p.ep_collect || (p.y_shared && !p.shared_gate))) return cudaErrorInvalidValue;

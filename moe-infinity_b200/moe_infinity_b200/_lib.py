@@ -16,6 +16,7 @@ DTYPE_BF16, DTYPE_F32, DTYPE_F16, DTYPE_FP8 = 0, 1, 2, 3
 EXPERT_SWITCH, EXPERT_SWITCH_GATED, EXPERT_NLLB, EXPERT_FSGPT, EXPERT_MIXTRAL, EXPERT_DEEPSEEK = 0, 1, 2, 3, 4, 5
 ROUTER_MIXTRAL, ROUTER_DEEPSEEK_GREEDY, ROUTER_DEEPSEEK_GROUP, ROUTER_SWITCH_TOP1, ROUTER_DEEPSEEK_V3 = 0, 1, 2, 3, 4
 ROUTER_QWEN_MOE = 5
+ROUTER_LLAMA4 = 6
 NUMERICS_REFERENCE, NUMERICS_FP32 = 0, 1
 CACHE_REFERENCE, CACHE_SLOTS, CACHE_ACTIVATION_AWARE = 0, 1, 2
 WEIGHTS_MODEL_DTYPE, WEIGHTS_FP8_E4M3_B128 = 0, 1

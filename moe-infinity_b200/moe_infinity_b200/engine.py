@@ -40,6 +40,9 @@ def _stream_ptr() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+# routers whose logits are an nn.Linear of the model: gate weight and logits in the model dtype
+_MODEL_DTYPE_ROUTERS = (L.ROUTER_MIXTRAL, L.ROUTER_QWEN_MOE, L.ROUTER_LLAMA4)
+
 class MoEEngine:
     def __init__(self, *, num_layers: int, num_experts: int, hidden: int, inter: int, top_k: int,
                  dtype: torch.dtype = torch.bfloat16, expert_type: int = L.EXPERT_MIXTRAL,
@@ -75,8 +78,8 @@ class MoEEngine:
         self.shared_inter = shared_inter
         self.expert_type = expert_type
         self.router = router
-        # Mixtral and Qwen routers are nn.Linear layers of the model: their weight is in the model dtype
-        gate_dtype = gate_dtype or (dtype if router in (L.ROUTER_MIXTRAL, L.ROUTER_QWEN_MOE) else torch.float32)
+        # Mixtral, Qwen and Llama 4 routers are nn.Linear layers of the model: their weight is in the model dtype
+        gate_dtype = gate_dtype or (dtype if router in _MODEL_DTYPE_ROUTERS else torch.float32)
         self.gate_dtype = gate_dtype
         cfg = L.Config()
         cfg.struct_size = C.sizeof(L.Config)
@@ -394,7 +397,7 @@ class MoEEngine:
         p = C.c_void_p()
         self._ck(self.lib.b2m_ws_ptr(self._h, L.WS[name], C.byref(p)))
         k, E, H, I = self.k, self.E, self.H, self.I
-        logits_dt = self.dtype if self.router in (L.ROUTER_MIXTRAL, L.ROUTER_QWEN_MOE) else torch.float32
+        logits_dt = self.dtype if self.router in _MODEL_DTYPE_ROUTERS else torch.float32
         shape, dt = {
             "topk_idx": ((T, k), torch.int32), "topk_w": ((T, k), torch.float32), "row_of": ((T, k), torch.int32),
             "perm_token": ((T * k,), torch.int32), "counts": ((E,), torch.int32), "offsets": ((E + 1,), torch.int32),

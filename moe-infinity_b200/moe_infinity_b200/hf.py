@@ -1,6 +1,7 @@
-"""HuggingFace plug-in helpers: run a `transformers` Mixtral, DeepSeek-V3, Qwen2-MoE or Qwen3-MoE model with its MoE blocks
-executed by the CUDA engine (`patch_mixtral`, `patch_deepseek_v3`, `patch_qwen_moe`), and load the routed experts of a published AWQ / GPTQ 4-bit checkpoint into
-an f16 int4 engine as they are stored (`load_int4_checkpoint`).
+"""HuggingFace plug-in helpers: run a `transformers` Mixtral, DeepSeek-V3, Qwen2-MoE, Qwen3-MoE or Llama 4 model with its MoE
+blocks executed by the CUDA engine (`patch_mixtral`, `patch_deepseek_v3`, `patch_qwen_moe`, `patch_llama4`), and load the
+routed experts of a published AWQ / GPTQ 4-bit checkpoint into an f16 int4 engine as they are stored
+(`load_int4_checkpoint`).
 
 The reference achieves this by monkey-patching HF classes at load time (moe_infinity/runtime/model_offload.py:285-321:
 `MixtralSparseMoeBlock -> SyncMixtralSparseMoeBlock`).  The installed transformers (5.x) stores the experts of a layer as
@@ -196,6 +197,71 @@ def patch_qwen_moe(model, max_tokens: int = 4096, num_slots: int = 0, device_mem
             engine.register_shared(l, [sh.gate_proj.weight.data, sh.up_proj.weight.data, sh.down_proj.weight.data])
             engine.set_shared_gate(l, moe.shared_expert_gate.weight.data)
         layers[l].mlp = B200QwenMoeAdapter(engine, l, moe.gate.weight.data)
+    return engine
+
+
+class B200Llama4MoeAdapter(nn.Module):
+    """Drop-in for transformers>=5 `Llama4TextMoe`: forward(hidden[..., H]) -> (out [T, H], router_logits [T, E]), the
+    tuple the Llama 4 decoder layer unpacks.  The router GEMM stays in PyTorch (`F.linear` in the model dtype, the logits
+    HF's Llama4Router computes and returns); the top-k, the sigmoid weights, the scaling of the expert inputs, the routed
+    experts, the shared expert and the combine run in the engine."""
+
+    def __init__(self, engine: MoEEngine, layer_id: int, gate_weight: torch.Tensor):
+        super().__init__()
+        self.engine = engine
+        self.layer_id = layer_id
+        self.gate_weight = nn.Parameter(gate_weight.detach().clone(), requires_grad=False)
+
+    def forward(self, hidden_states: torch.Tensor):
+        x = hidden_states.reshape(-1, hidden_states.shape[-1])
+        router_logits = F.linear(x, self.gate_weight)
+        return self.engine.forward(self.layer_id, x, router_logits=router_logits), router_logits
+
+
+def _is_llama4_moe(ff) -> bool:
+    try:
+        from transformers.models.llama4.modeling_llama4 import Llama4TextMoe
+    except ImportError:
+        return False
+    return isinstance(ff, Llama4TextMoe)
+
+
+def patch_llama4(model, max_tokens: int = 4096, num_slots: int = 0, device_memory_ratio: float = 0.0,
+                 resident: bool = True, engine: Optional[MoEEngine] = None) -> MoEEngine:
+    """Move the routed and shared experts of `model` (a transformers>=5 Llama4ForCausalLM, or the text model of a
+    Llama4ForConditionalGeneration, on a CUDA device) into a MoEEngine (ROUTER_LLAMA4, gate|up|down experts) and replace
+    its `Llama4TextMoe` blocks.  Only layers whose `feed_forward` is that block are replaced, so the dense layers Maverick
+    interleaves (`interleave_moe_layer_step`) stay.  Llama4TextExperts stores an expert's weights fused and transposed:
+    gate = gate_up_proj[e][:, :I].T, up = gate_up_proj[e][:, I:].T, down = down_proj[e].T.  `engine` may be given (built
+    with router=ROUTER_LLAMA4 and the model's shapes), e.g. one with expert_dtype=torch.float8_e4m3fn or torch.uint4: the
+    routed experts are then quantised with `fp8.quantize_block128` or `int4.quantize_g128`; the shared experts stay in the
+    model dtype.  `resident=False` registers the routed experts as pinned host blobs (offload mode, budget from num_slots
+    / device_memory_ratio)."""
+    cfg = model.config
+    cfg = getattr(cfg, "text_config", cfg)
+    layers = model.model.layers if hasattr(model, "model") else model.layers
+    dev = next(model.parameters()).device
+    dtype = next(model.parameters()).dtype
+    L_, E, H, I, k = len(layers), cfg.num_local_experts, cfg.hidden_size, cfg.intermediate_size, cfg.num_experts_per_tok
+    moe_layers = [l for l in range(L_) if _is_llama4_moe(layers[l].feed_forward)]
+    if engine is None:
+        engine = MoEEngine(num_layers=L_, num_experts=E, hidden=H, inter=I, top_k=k, dtype=dtype, expert_type=L.EXPERT_DEEPSEEK,
+                           router=L.ROUTER_LLAMA4, max_tokens=max_tokens,
+                           num_slots=(L_ * E if resident and not num_slots else num_slots),
+                           device_memory_ratio=device_memory_ratio, shared_inter=I, device=dev.index or 0)
+    elif engine.router != L.ROUTER_LLAMA4 or engine.expert_type != L.EXPERT_DEEPSEEK:
+        raise ValueError("patch_llama4 needs an engine built with router=ROUTER_LLAMA4 and expert_type=EXPERT_DEEPSEEK")
+    elif engine.shared_inter != I:
+        raise ValueError(f"the engine's shared_inter {engine.shared_inter} does not match the model's shared expert ({I})")
+    for l in moe_layers:
+        moe = layers[l].feed_forward
+        gu, dn = moe.experts.gate_up_proj.data, moe.experts.down_proj.data     # [E,H,2I], [E,I,H]
+        for e in range(E):
+            _load(engine, l, e, [gu[e, :, :I].t().contiguous(), gu[e, :, I:].t().contiguous(), dn[e].t().contiguous()],
+                  resident)
+        sh = moe.shared_expert
+        engine.register_shared(l, [sh.gate_proj.weight.data, sh.up_proj.weight.data, sh.down_proj.weight.data])
+        layers[l].feed_forward = B200Llama4MoeAdapter(engine, l, moe.router.weight.data)
     return engine
 
 
