@@ -100,6 +100,50 @@ const WeightFormat WEIGHT_FORMATS[] = {
     {B2M_WEIGHTS_INT4_G128_F16, "int4 (fp16 scales)", B2M_DTYPE_F16, 4, i4::grid_bytes, i4::GROUP, AS_INT4},
 };
 
+// How a router kind constrains the configuration and changes the host logic around its routing math (route.cu): one row
+// per B2M_ROUTER_* value.  ROUTER_DEEPSEEK_GROUP's group rule is checked at launch (route_args_ok), not here.
+enum : int { GROUPS_ANY = 0,   // n_group / topk_group are ignored
+             GROUPS_NONE = 1,  // no group-limited routing: n_group == topk_group == 1
+             GROUPS_V3 = 2 };  // noaux_tc: n_group in 1..32 divides E, E / n_group >= 2, topk_group in 1..n_group
+struct RouterKind {
+  int id;                     // B2M_ROUTER_*
+  const char* name;           // in messages
+  bool model_dtype_logits;    // the gate is an nn.Linear in the model dtype: logits are rounded to it (RouteParams)
+  bool gate_up_down;          // experts are gate|up|down (expert_type 5) ...
+  bool dtype16;               // ... in a bf16 or f16 model dtype
+  int groups;                 // GROUPS_*
+  bool unscaled;              // routed_scaling_factor must be 1
+  bool unnormalised;          // norm_topk_prob must be 0
+  bool needs_shared;          // every layer has a shared expert: shared_inter > 0
+  bool top1;                  // top_k must be 1
+  bool gate_bias;             // a per-layer correction bias (b2m_set_gate_bias), required to route and to look ahead
+  bool shared_gate;           // a per-layer shared-expert gate (b2m_set_shared_gate)
+  bool scales_inputs;         // the weights scale the gathered expert inputs and the combine sums unweighted; the router
+                              // ranks logits, so no scores as router input, and no input permutation
+  bool capacity;              // a capacity pass after top-k: seq_len divides T, extra routing launches, no early gate/up GEMM
+                              // and no direct-mode expert parallelism
+  bool ep;                    // expert parallelism is available
+  int combine, combine_fp32;  // COMBINE_* under B2M_NUMERICS_REFERENCE / B2M_NUMERICS_FP32
+};
+const RouterKind ROUTERS[] = {
+    // id, name, model_dtype_logits, gate_up_down, dtype16, groups, unscaled, unnormalised, needs_shared, top1, gate_bias,
+    // shared_gate, scales_inputs, capacity, ep, combine, combine_fp32
+    {B2M_ROUTER_MIXTRAL,        "mixtral",     true,  false, false, GROUPS_ANY,  false, false, false, false, false, false, false, false, true,  COMBINE_MIXTRAL,  COMBINE_FP32},
+    {B2M_ROUTER_DEEPSEEK_GREEDY, "greedy",     false, false, false, GROUPS_ANY,  false, false, false, false, false, false, false, false, true,  COMBINE_DEEPSEEK, COMBINE_FP32},
+    {B2M_ROUTER_DEEPSEEK_GROUP, "group",       false, false, false, GROUPS_ANY,  false, false, false, false, false, false, false, false, true,  COMBINE_DEEPSEEK, COMBINE_FP32},
+    {B2M_ROUTER_SWITCH_TOP1,    "switch",      false, false, false, GROUPS_ANY,  false, false, false, true,  false, false, false, true,  true,  COMBINE_SWITCH,   COMBINE_SWITCH},
+    {B2M_ROUTER_DEEPSEEK_V3,    "deepseek_v3", false, false, false, GROUPS_V3,   false, false, false, false, true,  false, false, false, true,  COMBINE_DEEPSEEK, COMBINE_FP32},
+    {B2M_ROUTER_QWEN_MOE,       "qwen_moe",    true,  true,  true,  GROUPS_NONE, true,  false, false, false, false, true,  false, false, false, COMBINE_QWEN,     COMBINE_FP32},
+    {B2M_ROUTER_LLAMA4,         "llama4",      true,  true,  true,  GROUPS_NONE, true,  true,  true,  false, false, false, true,  false, false, COMBINE_LLAMA4,   COMBINE_FP32},
+};
+// the names of the router kinds that have a feature, for the message that refuses it to the others
+std::string routers_with(bool RouterKind::*has) {
+  std::string s;
+  for (const RouterKind& r : ROUTERS)
+    if (r.*has) s += (s.empty() ? "" : " or ") + std::string(r.name);
+  return s;
+}
+
 struct Arena {
   uint8_t* base = nullptr;
   size_t slot_bytes = 0;
@@ -157,9 +201,9 @@ struct b2m_ctx {
   int* h_stage = nullptr;  // pinned [STAGE_RING][E]
   int stage_pos = 0;
   std::vector<const void*> gate_w;  // per layer device pointers
-  std::vector<const float*> gate_bias;  // B2M_ROUTER_DEEPSEEK_V3: per layer e_score_correction_bias [E] (device, borrowed)
+  std::vector<const float*> gate_bias;  // RouterKind::gate_bias: per layer e_score_correction_bias [E] (device, borrowed)
   std::vector<const uint16_t*> input_perm;  // B2M_WEIGHTS_INT4_G128_F16: per layer [E][H] gather table (device, borrowed) or null
-  std::vector<const void*> shared_gate_w;   // B2M_ROUTER_QWEN_MOE with shared experts: per layer [H] shared_expert_gate.weight
+  std::vector<const void*> shared_gate_w;   // RouterKind::shared_gate: per layer [H] shared_expert_gate.weight
 
   // workspace
   int cap_T = 0, cap_R = 0;
@@ -205,6 +249,7 @@ struct b2m_ctx {
 
   int cur_ksplit = 1, cur_nt = 16, cur_nt_dn = 16, cur_T = 0;   // token-tile widths of the up (K3) and down (K4) GEMMs
   const WeightFormat* wf = nullptr;   // how the routed experts are stored
+  const RouterKind* rk = nullptr;     // how they are routed
   bool ep_mode = false;       // experts of other ranks are simply absent (never an error)
   // 12-bit packed copy of the routed arena (weight_pack.cuh; same slot index), read by the decode GEMMs.  Allocated by the first
   // eager forward that packs, if the device keeps PK_RESERVE free beside it.  d_ok[slot]: bit b = matrix b (gate, up, down)
@@ -715,6 +760,7 @@ RouteParams base_route_params(b2m_ctx* c, int layer, const void* x, int T, int s
   p.T = T; p.H = f.hidden; p.E = f.num_experts; p.k = f.top_k;
   p.dtype = f.dtype;
   p.router = f.router;
+  p.logits_model_dtype = c->rk->model_dtype_logits;
   p.n_group = f.n_group; p.topk_group = f.topk_group; p.norm_topk_prob = f.norm_topk_prob;
   p.routed_scaling_factor = f.routed_scaling_factor;
   p.gate_bias = c->gate_bias[layer];
@@ -746,10 +792,17 @@ void plan_gemm(b2m_ctx* c, int T) {
 bool pdl_enabled() { return sw().pdl; }
 
 
-int route_launch_count(int T, int router, bool fused_gate) {
+int route_launch_count(int T, const RouterKind& rk, bool fused_gate) {
   if (T == 0) return 0;
   if (T <= 256) return 2;
-  return (router == B2M_ROUTER_SWITCH_TOP1 ? 5 : 3) + (fused_gate ? 1 : 0);
+  return (rk.capacity ? 5 : 3) + (fused_gate ? 1 : 0);
+}
+
+// scores as router input: a router that ranks its logits cannot take them
+int refuse_scores(b2m_ctx* c, int kind) {
+  if (kind == 2 && c->rk->scales_inputs)
+    return fail(c, B2M_EUNSUPPORTED, "%s router: takes logits (router_in_kind 0 or 1), not scores: it ranks the logits", c->rk->name);
+  return B2M_OK;
 }
 
 }  // namespace
@@ -796,52 +849,41 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       return fail(nullptr, B2M_EUNSUPPORTED, "%s weights run on the tensor-core GEMMs only (gemm_impl 1 is the bf16 cross-check kernel)",
                   wf->name);
   }
-  if (cfg->router < 0 || cfg->router > 6) return fail(nullptr, B2M_EINVAL, "bad router kind");
-  if (cfg->router == B2M_ROUTER_LLAMA4) {
-    if (cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: experts are gate|up|down (expert_type %d), got expert_type %d",
-                  B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, cfg->expert_type);
-    if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: the model dtype must be bf16 or f16, got dtype %d", cfg->dtype);
-    if (cfg->n_group != 1 || cfg->topk_group != 1)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: no group-limited routing (n_group=%d, topk_group=%d must be 1)",
-                  cfg->n_group, cfg->topk_group);
-    if (cfg->routed_scaling_factor != 1.0f)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: weights are not scaled (routed_scaling_factor=%g must be 1.0)",
-                  (double)cfg->routed_scaling_factor);
-    if (cfg->norm_topk_prob)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: weights are not normalised (norm_topk_prob=%d must be 0)",
-                  cfg->norm_topk_prob);
-    if (cfg->shared_inter <= 0)
-      return fail(nullptr, B2M_EINVAL, "llama4 router: every Llama 4 MoE layer has a shared expert (shared_inter=%d must be > 0)",
-                  cfg->shared_inter);
-  }
-  if (cfg->router == B2M_ROUTER_QWEN_MOE) {
-    if (cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
-      return fail(nullptr, B2M_EINVAL, "qwen_moe router: experts are gate|up|down (expert_type %d), got expert_type %d",
-                  B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, cfg->expert_type);
-    if (cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16)
-      return fail(nullptr, B2M_EINVAL, "qwen_moe router: the model dtype must be bf16 or f16, got dtype %d", cfg->dtype);
-    if (cfg->n_group != 1 || cfg->topk_group != 1)
-      return fail(nullptr, B2M_EINVAL, "qwen_moe router: no group-limited routing (n_group=%d, topk_group=%d must be 1)",
-                  cfg->n_group, cfg->topk_group);
-    if (cfg->routed_scaling_factor != 1.0f)
-      return fail(nullptr, B2M_EINVAL, "qwen_moe router: weights are not scaled (routed_scaling_factor=%g must be 1.0)",
-                  (double)cfg->routed_scaling_factor);
-  }
-  if (cfg->router == B2M_ROUTER_DEEPSEEK_V3) {
+  const RouterKind* rk = nullptr;
+  for (const RouterKind& r : ROUTERS)
+    if (r.id == cfg->router) rk = &r;
+  if (!rk) return fail(nullptr, B2M_EINVAL, "bad router kind");
+  if (rk->gate_up_down && cfg->expert_type != B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE)
+    return fail(nullptr, B2M_EINVAL, "%s router: experts are gate|up|down (expert_type %d), got expert_type %d", rk->name,
+                B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, cfg->expert_type);
+  if (rk->dtype16 && cfg->dtype != B2M_DTYPE_BF16 && cfg->dtype != B2M_DTYPE_F16)
+    return fail(nullptr, B2M_EINVAL, "%s router: the model dtype must be bf16 or f16, got dtype %d", rk->name, cfg->dtype);
+  if (rk->groups == GROUPS_NONE && (cfg->n_group != 1 || cfg->topk_group != 1))
+    return fail(nullptr, B2M_EINVAL, "%s router: no group-limited routing (n_group=%d, topk_group=%d must be 1)", rk->name,
+                cfg->n_group, cfg->topk_group);
+  if (rk->groups == GROUPS_V3) {
     if (cfg->n_group < 1 || cfg->n_group > 32 || cfg->num_experts % cfg->n_group)
-      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: n_group=%d must be in 1..32 and divide num_experts=%d", cfg->n_group,
-                  cfg->num_experts);
+      return fail(nullptr, B2M_EINVAL, "%s router: n_group=%d must be in 1..32 and divide num_experts=%d", rk->name,
+                  cfg->n_group, cfg->num_experts);
     if (cfg->num_experts / cfg->n_group < 2)
-      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: a group needs at least 2 experts (top-2 group score), got %d",
+      return fail(nullptr, B2M_EINVAL, "%s router: a group needs at least 2 experts (top-2 group score), got %d", rk->name,
                   cfg->num_experts / cfg->n_group);
     if (cfg->topk_group < 1 || cfg->topk_group > cfg->n_group)
-      return fail(nullptr, B2M_EINVAL, "deepseek_v3 router: topk_group=%d must be in 1..n_group=%d", cfg->topk_group, cfg->n_group);
+      return fail(nullptr, B2M_EINVAL, "%s router: topk_group=%d must be in 1..n_group=%d", rk->name, cfg->topk_group,
+                  cfg->n_group);
   }
+  if (rk->unscaled && cfg->routed_scaling_factor != 1.0f)
+    return fail(nullptr, B2M_EINVAL, "%s router: weights are not scaled (routed_scaling_factor=%g must be 1.0)", rk->name,
+                (double)cfg->routed_scaling_factor);
+  if (rk->unnormalised && cfg->norm_topk_prob)
+    return fail(nullptr, B2M_EINVAL, "%s router: weights are not normalised (norm_topk_prob=%d must be 0)", rk->name,
+                cfg->norm_topk_prob);
+  if (rk->needs_shared && cfg->shared_inter <= 0)
+    return fail(nullptr, B2M_EINVAL, "%s router: every MoE layer has a shared expert (shared_inter=%d must be > 0)", rk->name,
+                cfg->shared_inter);
+  if (rk->top1 && cfg->top_k != 1) return fail(nullptr, B2M_EINVAL, "%s router needs top_k=1", rk->name);
   if (cfg->cache_policy < B2M_CACHE_REFERENCE || cfg->cache_policy > B2M_CACHE_ACTIVATION_AWARE) return fail(nullptr, B2M_EINVAL, "bad cache_policy");
   if (cfg->freq_alpha < 0.f || cfg->freq_alpha > 1.f) return fail(nullptr, B2M_EINVAL, "freq_alpha must be in [0,1]");
-  if (cfg->router == B2M_ROUTER_SWITCH_TOP1 && cfg->top_k != 1) return fail(nullptr, B2M_EINVAL, "switch router needs top_k=1");
 
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -853,6 +895,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (!c) return fail(nullptr, B2M_ENOMEM, "out of host memory");
   c->cfg = *cfg;
   c->wf = wf;
+  c->rk = rk;
   memset(&c->stats, 0, sizeof c->stats);
 #define CKC(call)                                                                                     \
   do {                                                                                                \
@@ -967,7 +1010,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
     CKC(cudaMalloc(&c->d_hmid_s, (size_t)T * cfg->shared_inter * esize));
     CKC(cudaMemset(c->d_hmid_s, 0, (size_t)T * cfg->shared_inter * esize));
     CKC(cudaMalloc((void**)&c->d_y_s, (size_t)T * H * sizeof(float)));
-    if (cfg->router == B2M_ROUTER_QWEN_MOE) CKC(cudaMalloc(&c->d_shared_gate, (size_t)T * esize));
+    if (rk->shared_gate) CKC(cudaMalloc(&c->d_shared_gate, (size_t)T * esize));
   }
   for (int i = 0; tc && i < 5; ++i) {
     r = build_act_map(c, &c->tm_xp[i], c->d_xp, H, (int)R, NT_LIST[i]);
@@ -1090,9 +1133,9 @@ int b2m_set_gate(b2m_ctx* c, int layer, const void* dev_gate_weight) {
 int b2m_set_gate_bias(b2m_ctx* c, int layer, const float* dev_bias) {
   int r = check_layer(c, layer);
   if (r) return r;
-  if (c->cfg.router != B2M_ROUTER_DEEPSEEK_V3)
-    return fail(c, B2M_EINVAL, "b2m_set_gate_bias: only a deepseek_v3 router (%d) has a correction bias, this context's router is %d",
-                B2M_ROUTER_DEEPSEEK_V3, c->cfg.router);
+  if (!c->rk->gate_bias)
+    return fail(c, B2M_EINVAL, "b2m_set_gate_bias: only a %s router has a correction bias, this context's router is %s",
+                routers_with(&RouterKind::gate_bias).c_str(), c->rk->name);
   if (!dev_bias) return fail(c, B2M_EINVAL, "b2m_set_gate_bias: dev_bias is null");
   c->gate_bias[layer] = dev_bias;
   return B2M_OK;
@@ -1101,9 +1144,9 @@ int b2m_set_gate_bias(b2m_ctx* c, int layer, const float* dev_bias) {
 int b2m_set_shared_gate(b2m_ctx* c, int layer, const void* dev_w) {
   int r = check_layer(c, layer);
   if (r) return r;
-  if (c->cfg.router != B2M_ROUTER_QWEN_MOE)
-    return fail(c, B2M_EINVAL, "b2m_set_shared_gate: only a qwen_moe router (%d) has a shared-expert gate, this context's router is %d",
-                B2M_ROUTER_QWEN_MOE, c->cfg.router);
+  if (!c->rk->shared_gate)
+    return fail(c, B2M_EINVAL, "b2m_set_shared_gate: only a %s router has a shared-expert gate, this context's router is %s",
+                routers_with(&RouterKind::shared_gate).c_str(), c->rk->name);
   if (c->cfg.shared_inter <= 0) return fail(c, B2M_EINVAL, "b2m_set_shared_gate: the context has no shared experts (shared_inter = 0)");
   if (!dev_w) return fail(c, B2M_EINVAL, "b2m_set_shared_gate: dev_w is null");
   c->shared_gate_w[layer] = dev_w;
@@ -1113,8 +1156,8 @@ int b2m_set_shared_gate(b2m_ctx* c, int layer, const void* dev_w) {
 int b2m_set_input_perm(b2m_ctx* c, int layer, const uint16_t* dev_perm) {
   int r = check_layer(c, layer);
   if (r) return r;
-  if (c->cfg.router == B2M_ROUTER_LLAMA4)
-    return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations are not available with the llama4 router");
+  if (c->rk->scales_inputs)
+    return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations are not available with the %s router", c->rk->name);
   if (c->wf->id != B2M_WEIGHTS_INT4_G128_F16)
     return fail(c, B2M_EUNSUPPORTED, "b2m_set_input_perm: input permutations (act-order GPTQ) need a B2M_WEIGHTS_INT4_G128_F16 "
                 "context");
@@ -1237,13 +1280,13 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
     p.logits_dtype = in_dtype;
     p.logits_are_scores = (kind == 2);
     if (kind == 2 && in_dtype != B2M_DTYPE_F32) return fail(c, B2M_EINVAL, "scores must be fp32");
-    if (kind == 2 && c->cfg.router == B2M_ROUTER_LLAMA4)
-      return fail(c, B2M_EUNSUPPORTED, "llama4 router: takes logits (router_in_kind 0 or 1), not scores: it ranks the logits");
+    r = refuse_scores(c, kind);
+    if (r) return r;
   }
-  p.scale_rows = c->cfg.router == B2M_ROUTER_LLAMA4;   // the routing weight scales the expert's input row
-  if (c->cfg.router == B2M_ROUTER_SWITCH_TOP1 && (p.seq_len <= 0 || T % p.seq_len))
+  p.scale_rows = c->rk->scales_inputs;   // the routing weight scales the expert's input row
+  if (c->rk->capacity && (p.seq_len <= 0 || T % p.seq_len))
     return fail(c, B2M_EINVAL, "T=%d is not a multiple of seq_len=%d", T, p.seq_len);
-  if (c->cfg.router == B2M_ROUTER_DEEPSEEK_V3 && !p.gate_bias)
+  if (c->rk->gate_bias && !p.gate_bias)
     return fail(c, B2M_ESTATE, "layer %d has no correction bias (b2m_set_gate_bias)", layer);
   plan_gemm(c, T);
   if (c->cur_ksplit > 1) { p.y_zero = c->d_y; p.y_zero_elems = (size_t)T * c->cfg.top_k * c->cfg.hidden; }
@@ -1253,7 +1296,7 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
   // Not with B2M_PDL=1: with a programmatic edge on EVERY kernel the permute kernel may start before the gate/top-k kernel
   // has finished, so a GEMM that reads offsets/slot_of before its own griddepcontrol.wait could see the previous layer's
   // tables.  Pre-wait reads may only touch data older than the predecessor's own launch.
-  c->k3_early_ok = k3_early && !pdl_enabled() && T >= 1 && T <= 256 && c->cfg.router != B2M_ROUTER_SWITCH_TOP1 && !ep_dispatch &&
+  c->k3_early_ok = k3_early && !pdl_enabled() && T >= 1 && T <= 256 && !c->rk->capacity && !ep_dispatch &&
                    !c->offload && !c->ep_mode && c->cfg.gemm_impl != 1;
   p.offsets_early = c->k3_early_ok ? 1 : 0;
   const bool rows_by_gate = sw().rows_by_gate;
@@ -1268,7 +1311,7 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
     p.y_zero = nullptr;        // the regroup kernel (direct mode: the owner's gate/up GEMM) clears the accumulator
   }
   CK(c, launch_route(p, st));
-  c->stats.kernel_launches += route_launch_count(T, c->cfg.router, kind == 0) - (p.ep_fused ? 1 : 0);
+  c->stats.kernel_launches += route_launch_count(T, *c->rk, kind == 0) - (p.ep_fused ? 1 : 0);
   c->ep_fused_last = p.ep_fused != 0;
   c->last_counts_valid = false;
   // router-logit driven prefetch: the next layer's router applied to THIS layer's input predicts which experts the next
@@ -1277,7 +1320,7 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
   c->look_pending = false;
   const int nxt = (layer + 1) % c->cfg.num_layers;
   if (c->cfg.lookahead_prefetch && c->offload && !c->ep_mode && T >= 1 && T <= 256 && c->cfg.dtype != B2M_DTYPE_F32 &&
-      c->cfg.num_layers > 1 && c->gate_w[nxt] && (c->cfg.router != B2M_ROUTER_DEEPSEEK_V3 || c->gate_bias[nxt])) {
+      c->cfg.num_layers > 1 && c->gate_w[nxt] && (!c->rk->gate_bias || c->gate_bias[nxt])) {
     RouteParams q = p;
     q.gate_w = c->gate_w[nxt];
     q.gate_bias = c->gate_bias[nxt];
@@ -1699,12 +1742,8 @@ static int combine_impl(b2m_ctx* c, int layer, const void* x, int T, void* out, 
   p.topk_idx = c->d_topk_idx; p.topk_w = c->d_topk_w; p.row_of = c->d_row_of;
   p.out = out;
   p.T = T; p.H = f.hidden; p.k = f.top_k; p.dtype = f.dtype;
-  if (f.router == B2M_ROUTER_SWITCH_TOP1) p.mode = COMBINE_SWITCH;
-  else if (f.numerics == B2M_NUMERICS_FP32) p.mode = COMBINE_FP32;
-  else if (f.router == B2M_ROUTER_QWEN_MOE) p.mode = COMBINE_QWEN;
-  else if (f.router == B2M_ROUTER_LLAMA4) p.mode = COMBINE_LLAMA4;
-  else p.mode = f.router == B2M_ROUTER_MIXTRAL ? COMBINE_MIXTRAL : COMBINE_DEEPSEEK;
-  p.unweighted = f.router == B2M_ROUTER_LLAMA4;   // the weights scaled the expert inputs (COMBINE_LLAMA4 or COMBINE_FP32)
+  p.mode = f.numerics == B2M_NUMERICS_FP32 ? c->rk->combine_fp32 : c->rk->combine;
+  p.unweighted = c->rk->scales_inputs;   // the weights scaled the expert inputs (COMBINE_LLAMA4 or COMBINE_FP32)
   if (f.shared_inter > 0) {
     if (c->shared_in_flight) {
       // launched by b2m_moe_forward on the side stream at the start of the call: join it
@@ -1733,8 +1772,8 @@ int b2m_moe_forward(b2m_ctx* c, int layer, const void* x, const void* router_in,
                     int seq_len, void* out, void* stream) {
   int r = check_layer(c, layer);
   if (r) return r;
-  if (kind == 2 && c->cfg.router == B2M_ROUTER_LLAMA4)   // refused before the shared expert is launched
-    return fail(c, B2M_EUNSUPPORTED, "llama4 router: takes logits (router_in_kind 0 or 1), not scores: it ranks the logits");
+  r = refuse_scores(c, kind);   // before the shared expert is launched
+  if (r) return r;
   if (c->cfg.shared_inter > 0 && T > 0 && T <= c->cap_T && x) {
     // the shared experts (deepseek.py:133-136) depend on x only: fork them onto a side stream so that their two GEMM
     // launches overlap the gate / top-k / permute kernels of the routed path; b2m_combine joins
@@ -1906,8 +1945,7 @@ static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (!c) return B2M_EINVAL;
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
   if (c->wf->a_src != AS_BF16) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with %s weights", c->wf->name);
-  if (c->cfg.router == B2M_ROUTER_QWEN_MOE) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the qwen_moe router");
-  if (c->cfg.router == B2M_ROUTER_LLAMA4) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the llama4 router");
+  if (!c->rk->ep) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the %s router", c->rk->name);
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
     return fail(c, B2M_EINVAL, "bad expert-parallel geometry (nranks=%d rank=%d cap=%d E=%d)", nranks, rank, cap, c->cfg.num_experts);
   if ((long long)nranks * cap > c->cap_R)
@@ -2123,7 +2161,7 @@ int b2m_ep_p2p_layer(b2m_ctx* c, int layer, const void* x, const void* router_in
   const bool direct_on = sw().ep_direct;
   // direct mode: the fused route+dispatch kernel needs every CTA resident (T_local <= #SMs)
   const bool direct = direct_on && T_local <= c->num_sms && f.gemm_impl != 1 && f.shared_inter == 0 &&
-                      f.router != B2M_ROUTER_SWITCH_TOP1 && f.dtype != B2M_DTYPE_F32;
+                      !c->rk->capacity && f.dtype != B2M_DTYPE_F32;
   cudaStream_t st = (cudaStream_t)stream;
   if (!direct) {
     r = b2m_ep_p2p_route(c, layer, x, router_in, kind, in_dtype, T_local, stream);

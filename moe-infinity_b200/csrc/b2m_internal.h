@@ -220,6 +220,7 @@ struct RouteParams {
   EpParams ep;
   unsigned long long* tl;    // optional timeline slots: [0] gate/top-k start, [1] its end, [2] permute start, [3] permute end
   int scale_rows;            // Llama 4: the gathered row of pair i is round(x[t] * topk_w[i]) (written by this routing call)
+  int logits_model_dtype;    // the router's logits are rounded to the model dtype (its gate is an nn.Linear in that dtype)
 };
 cudaError_t launch_route(const RouteParams& p, cudaStream_t st);
 // look-ahead: top-k of the NEXT layer's router (p.gate_w = its weight; DeepSeek-V3: p.gate_bias = its bias) on this layer's

@@ -31,15 +31,6 @@ __device__ __forceinline__ float load_as_float(const void* p, size_t i, int dt) 
 }
 // bytes of one hidden row of the model dtype (fp32 models: 4-byte elements; rows stay multiples of 16 B since H % 8 == 0)
 __device__ __forceinline__ size_t row_bytes(const RouteParams& p) { return (size_t)p.H * (p.dtype == DT_F32 ? 4 : 2); }
-// Routers whose gate is an nn.Linear in the model dtype: their logits are rounded to the model dtype before the softmax
-// (Mixtral, mixtral.py:46; Qwen2-MoE / Qwen3-MoE, modeling_qwen2_moe.py Qwen2MoeTopKRouter; Llama 4, Llama4Router, which
-// ranks those logits directly).  The others take fp32 logits.  Written as two compares (the router kinds from
-// ROUTER_QWEN_MOE on all take model-dtype logits; b2m_ctx_create_ex admits none above ROUTER_LLAMA4), so that the unrolled
-// gate loops of the other routers compile to the code they had before Llama 4.
-static_assert(ROUTER_LLAMA4 == ROUTER_QWEN_MOE + 1, "logits_in_model_dtype: every router from ROUTER_QWEN_MOE on has model-dtype logits");
-__host__ __device__ __forceinline__ bool logits_in_model_dtype(int router) {
-  return router == ROUTER_MIXTRAL || router >= ROUTER_QWEN_MOE;
-}
 __device__ __forceinline__ float round_to(float f, int dt) {
   if (dt == DT_BF16) return round_dt<DT_BF16>(f);
   if (dt == DT_F16) return round_dt<DT_F16>(f);
@@ -68,7 +59,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // --------------------------------------------------------------------------------------
 // K0: router gate.  logits[e] = <x[t], Wg[e]> with fp32 accumulation, 16-byte vector loads.
-// Mixtral: nn.Linear in model dtype -> result rounded to the model dtype (mixtral.py:46).
+// p.logits_model_dtype (Mixtral, mixtral.py:46; Qwen2-MoE / Qwen3-MoE, Qwen2MoeTopKRouter; Llama 4, Llama4Router, which
+// ranks those logits directly): nn.Linear in model dtype -> result rounded to the model dtype.
 // DeepSeek/Switch: fp32 linear on upcast operands (modeling_deepseek.py:467-471).
 // --------------------------------------------------------------------------------------
 __device__ __forceinline__ void unpack8(const uint4& v, int dt, float (&f)[8]) {
@@ -106,7 +98,7 @@ __device__ float gate_dot_warp(const RouteParams& p, int t, int e) {
     }
   }
   acc = warp_sum(acc);
-  return logits_in_model_dtype(p.router) ? round_to(acc, p.dtype) : acc;
+  return round_to(acc, p.logits_model_dtype ? p.dtype : DT_F32);
 }
 // One warp, one token, experts [e0, e0+8): x is loaded once per 8-element chunk and reused for all 8 rows
 // (16-byte loads of both operands).  out[i] (i < 8) valid in every lane.  No predicates inside the loop (expert
@@ -148,7 +140,7 @@ __device__ __forceinline__ void gate_dot8_impl(const RouteParams& p, int t, int 
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const float v = warp_sum(acc[i]);
-    out[i] = logits_in_model_dtype(p.router) ? round_to(v, p.dtype) : v;
+    out[i] = round_to(v, p.logits_model_dtype ? p.dtype : DT_F32);
   }
 }
 __device__ __forceinline__ void gate_dot8_warp(const RouteParams& p, int t, int e0, float (&out)[8]) {
@@ -267,7 +259,7 @@ __device__ __forceinline__ void gate_logits_impl(const RouteParams& p, uint4* ri
           const float v = warp_sum(acc[q][i]);
           const int t = t0 + q;
           if (lane == 0 && t < p.T && e0 + i < p.E) {
-            if (logits_in_model_dtype(p.router))
+            if (p.logits_model_dtype)
               reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e0 + i] =
                   p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(v) : Half16<DT_F16>::from_f(v);
             else
@@ -724,7 +716,7 @@ __global__ void __launch_bounds__(RT_THREADS) route_topk_kernel(const RouteParam
     if (p.logits_out && !scores_in) {
       for (int e = lane; e < p.E; e += 32) {
         const float lv = s_logits[warp][e];
-        if (logits_in_model_dtype(p.router)) {
+        if (p.logits_model_dtype) {
           reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e] =
               p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(lv) : Half16<DT_F16>::from_f(lv);
         } else {
@@ -895,7 +887,7 @@ __global__ void __launch_bounds__(RT_THREADS) gate_topk_small_kernel(const Route
     if (p.logits_out && !scores_in) {
       for (int e = lane; e < p.E; e += 32) {
         const float lv = s_logits[e];
-        if (logits_in_model_dtype(p.router))
+        if (p.logits_model_dtype)
           reinterpret_cast<uint16_t*>(p.logits_out)[(size_t)t * p.E + e] =
               p.dtype == DT_BF16 ? Half16<DT_BF16>::from_f(lv) : Half16<DT_F16>::from_f(lv);
         else
@@ -1236,7 +1228,7 @@ cudaError_t launch_route(const RouteParams& p, cudaStream_t st) {
       gate_logits_kernel<<<dim3(nblocks, gsplit), 256, 0, st>>>(p);
     }
     q.logits = p.logits_out;
-    q.logits_dtype = logits_in_model_dtype(p.router) ? p.dtype : DT_F32;
+    q.logits_dtype = p.logits_model_dtype ? p.dtype : DT_F32;
     q.logits_are_scores = 0;
     q.logits_out = nullptr;
   }
@@ -1272,13 +1264,23 @@ cudaError_t launch_route_from_mask(const RouteParams& p, const uint8_t* mask, cu
 // K5: un-permute + weighted combine.  One warp-group of lanes shares a token's (row, weight) list by
 // warp shuffle; every lane owns 8 consecutive hidden elements (2 x 16 B fp32 loads per expert row,
 // one 16 B store).  Experts are applied in ascending expert id (the oracle's fixed order).
-// QWEN: the instantiation for Qwen2-MoE / Qwen3-MoE layers (COMBINE_QWEN, or COMBINE_FP32 with a gated shared expert); the
-// other instantiation compiles exactly the code it had before that mode existed.
+// RULE: which combine arithmetic the instantiation compiles (launch_combine picks it):
+//   RULE_PLAIN   COMBINE_MIXTRAL / DEEPSEEK / SWITCH / FP32, and the expert-parallel collect path;
+//   RULE_QWEN    Qwen2-MoE / Qwen3-MoE layers (COMBINE_QWEN, or COMBINE_FP32 with a gated shared expert);
+//   RULE_LLAMA4  Llama 4 layers (COMBINE_LLAMA4, or COMBINE_FP32): the routing weights already scaled the expert inputs, so
+//                the expert outputs are summed without weights -- routed_out.reshape(k, T, H).sum(dim=0) on the model dtype
+//                accumulates round(y) in fp32 and rounds once -- and out = shared_expert(x).add_(that sum):
+//                round(r + round(s)).  COMBINE_FP32: round(sum of y + s).  Experts in ascending id, as in the dense HF
+//                sum (its unselected experts add exact zeros).  No weights are loaded and there is no collect path.
+// Each branch on RULE is decided at compile time, so the plain and Qwen instantiations compile exactly the code they had
+// before the Qwen and Llama 4 rules existed.
 // --------------------------------------------------------------------------------------
 constexpr int CB_THREADS = 256;
+enum : int { RULE_PLAIN = 0, RULE_QWEN = 1, RULE_LLAMA4 = 2 };
 
-template <int DT, bool QWEN>
+template <int DT, int RULE>
 __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams p) {
+  constexpr bool WEIGHTED = RULE != RULE_LLAMA4;   // also: may collect expert-parallel outputs
   const int t = blockIdx.x;
   const int lane = threadIdx.x & 31;
   const int k = p.k;
@@ -1286,14 +1288,14 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
   // expert parallel, direct mode: launched with a programmatic edge behind the down GEMM and NOT waiting for that grid to
   // drain -- everything it reads from earlier kernels is older than the GEMMs (routing tables) and the expert outputs are
   // guarded by the owners' "done" flags (this rank's own included), so its CTAs are resident and polling when "done" lands
-  if (!(p.ep_collect && p.ep.direct && p.ep_early)) pdl_wait();
+  if (!(WEIGHTED && p.ep_collect && p.ep.direct && p.ep_early)) pdl_wait();
   if (p.tl && threadIdx.x == 0) tl_min(p.tl);
   // each warp loads the token's routing list into lanes 0..k-1 and sorts it by expert id via shuffles
   int my_e = 0x7fffffff, my_row = -1;
   float my_w = 0.f;
   if (lane < k) {
     my_e = p.topk_idx[(size_t)t * k + lane];
-    my_w = p.topk_w[(size_t)t * k + lane];
+    if (WEIGHTED) my_w = p.topk_w[(size_t)t * k + lane];
     my_row = p.row_of[(size_t)t * k + lane];
     if (my_e < 0 || my_row < 0) { my_e = 0x7ffffff0 + lane; my_row = -1; }
   }
@@ -1307,7 +1309,7 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
   const uint16_t* src16[MAX_K];
   const float* srcf[MAX_K];
   int my_owner = 0;
-  if (p.ep_collect) {
+  if (WEIGHTED && p.ep_collect) {
     if (p.ep.p2p) p2p_wait(p.ep, 1, (p.ep.direct && p.ep_early) ? 0 : -1);   // return rows landed (direct mode: the owners' GEMMs are done)
     if (p.tl && threadIdx.x == 0) tl_max(p.tl + 1);
     if (lane < k && my_row >= 0) {
@@ -1330,9 +1332,9 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
       const uint32_t who = __ballot_sync(0xffffffffu, lane < k && rank == r);
       const int src = __ffs(who) - 1;
       rows[r] = __shfl_sync(0xffffffffu, my_row, src);
-      ws[r] = __shfl_sync(0xffffffffu, my_w, src);
+      if (WEIGHTED) ws[r] = __shfl_sync(0xffffffffu, my_w, src);
       const int owner = __shfl_sync(0xffffffffu, my_owner, src);
-      if (p.ep_collect && rows[r] >= 0) {
+      if (WEIGHTED && p.ep_collect && rows[r] >= 0) {
         if (p.ep.direct) srcf[r] = p.ep.peer_y[owner] + (size_t)rows[r] * p.H;   // the owner's fp32 outputs, read over NVLink
         else src16[r] = reinterpret_cast<const uint16_t*>(p.ep.back_rows) + (size_t)rows[r] * p.H;
       }
@@ -1355,12 +1357,12 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
         const int r = r0 + q;
         if (r < k) {
           const bool ok = rows[r] >= 0;
-          if (p.ep_collect && p.ep.direct) {
+          if (WEIGHTED && p.ep_collect && p.ep.direct) {
             const float4* src = reinterpret_cast<const float4*>((ok ? srcf[r] : p.ep.local_y) + h);
             const float4 a = src[0], b = src[1];
             yk[q][0] = a.x; yk[q][1] = a.y; yk[q][2] = a.z; yk[q][3] = a.w;
             yk[q][4] = b.x; yk[q][5] = b.y; yk[q][6] = b.z; yk[q][7] = b.w;
-          } else if (p.ep_collect) {
+          } else if (WEIGHTED && p.ep_collect) {
             const uint16_t* sp = ok ? src16[r] : reinterpret_cast<const uint16_t*>(p.ep.back_rows);
             const uint4 v = *reinterpret_cast<const uint4*>(sp + h);
             const uint16_t* vs = reinterpret_cast<const uint16_t*>(&v);
@@ -1382,7 +1384,9 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
           const float w = ws[r];
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            if (p.mode == COMBINE_FP32) {
+            if (RULE == RULE_LLAMA4) {
+              acc[i] = __fadd_rn(acc[i], p.mode == COMBINE_FP32 ? y[i] : round_dt<DT>(y[i]));
+            } else if (p.mode == COMBINE_FP32) {
               acc[i] = fmaf(y[i], w, acc[i]);
             } else if (p.mode == COMBINE_MIXTRAL) {
               // out (model dtype) * weight (model dtype) -> rounded; final += -> rounded  (mixtral.py:98-101)
@@ -1392,7 +1396,7 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
               // out (model dtype) * weight (fp32) -> fp32; final(model dtype) += fp32 -> rounded (deepseek.py:125-128)
               const float prod = __fmul_rn(round_dt<DT>(y[i]), w);
               acc[i] = round_dt<DT>(__fadd_rn(acc[i], prod));
-            } else if (QWEN) {   // COMBINE_QWEN
+            } else if (RULE == RULE_QWEN) {   // COMBINE_QWEN
               // Qwen2MoeExperts: index_add_(final (model dtype, zeros), (out (model dtype) * weight (fp32)).to(model dtype)):
               // the product is rounded, then every add is rounded
               const float prod = round_dt<DT>(__fmul_rn(round_dt<DT>(y[i]), w));
@@ -1405,7 +1409,7 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
         }
       }
     }
-    if (p.mode == COMBINE_SWITCH) {
+    if (WEIGHTED && p.mode == COMBINE_SWITCH) {
       // dropped tokens keep their input; hidden = router_probs * next_states (switch_transformers.py:81,109)
       const uint4 xv = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.x) + (size_t)t * H + h);
       const uint16_t* xs = reinterpret_cast<const uint16_t*>(&xv);
@@ -1420,7 +1424,7 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
       const float4* src = reinterpret_cast<const float4*>(p.y_shared + (size_t)t * H + h);
       const float4 a = src[0], b = src[1];
       const float s[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-      if (QWEN) {
+      if (RULE == RULE_QWEN) {
         // Qwen2MoeSparseMoeBlock: out + sigmoid(shared_expert_gate(x)) * shared_expert(x), every op in the model dtype;
         // g = that sigmoid, already rounded (shared_gate_kernel)
         const float g = Half16<DT>::to_f(p.shared_gate[t]);
@@ -1429,6 +1433,10 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
           if (p.mode == COMBINE_FP32) acc[i] = fmaf(g, s[i], acc[i]);
           else acc[i] = round_dt<DT>(__fadd_rn(acc[i], round_dt<DT>(__fmul_rn(g, round_dt<DT>(s[i])))));
         }
+      } else if (RULE == RULE_LLAMA4) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          acc[i] = p.mode == COMBINE_FP32 ? __fadd_rn(acc[i], s[i]) : __fadd_rn(round_dt<DT>(acc[i]), round_dt<DT>(s[i]));
       } else {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -1446,84 +1454,15 @@ __global__ void __launch_bounds__(CB_THREADS) combine_kernel(const CombineParams
   if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
 }
 
-// --------------------------------------------------------------------------------------
-// Llama 4 combine (Llama4TextMoe.forward): the routing weights already scaled the expert inputs, so the expert outputs are
-// summed without weights -- routed_out.reshape(k, T, H).sum(dim=0) on the model dtype accumulates round(y) in fp32 and
-// rounds once -- and out = shared_expert(x).add_(that sum): round(r + round(s)).  COMBINE_FP32: round(sum of y + s).
-// Experts in ascending id, as in the dense HF sum (its unselected experts add exact zeros).  A kernel of its own, so the
-// instantiations of combine_kernel compile exactly the code they had before this mode existed.
-// --------------------------------------------------------------------------------------
-template <int DT>
-__global__ void __launch_bounds__(CB_THREADS) combine_llama4_kernel(const CombineParams p) {
-  const int t = blockIdx.x;
-  const int lane = threadIdx.x & 31;
-  const int k = p.k;
-  pdl_launch();
-  pdl_wait();
-  if (p.tl && threadIdx.x == 0) tl_min(p.tl);
-  int my_e = 0x7fffffff, my_row = -1;
-  if (lane < k) {
-    my_e = p.topk_idx[(size_t)t * k + lane];
-    my_row = p.row_of[(size_t)t * k + lane];
-    if (my_e < 0 || my_row < 0) { my_e = 0x7ffffff0 + lane; my_row = -1; }
-  }
-  int rank = 0;
-  for (int j = 0; j < k; ++j) rank += (__shfl_sync(0xffffffffu, my_e, j) < my_e) ? 1 : 0;
-  int rows[MAX_K];
-#pragma unroll
-  for (int r = 0; r < MAX_K; ++r) {
-    rows[r] = -1;
-    if (r < k) {
-      const uint32_t who = __ballot_sync(0xffffffffu, lane < k && rank == r);
-      rows[r] = __shfl_sync(0xffffffffu, my_row, __ffs(who) - 1);
-    }
-  }
-  const bool fp32 = p.mode == COMBINE_FP32;
-  const int H = p.H;
-  for (int h = (blockIdx.y * CB_THREADS + threadIdx.x) * 8; h < H; h += gridDim.y * CB_THREADS * 8) {
-    float acc[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-    // four expert rows in flight at a time (invalid rows read row 0 and are ignored), as in combine_kernel
-#pragma unroll
-    for (int r0 = 0; r0 < MAX_K; r0 += 4) {
-      if (r0 >= k) break;
-      float yk[4][8];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int r = r0 + q;
-        if (r < k) {
-          const float4* src = reinterpret_cast<const float4*>(p.y + (size_t)(rows[r] >= 0 ? rows[r] : 0) * H + h);
-          const float4 a = src[0], b = src[1];
-          yk[q][0] = a.x; yk[q][1] = a.y; yk[q][2] = a.z; yk[q][3] = a.w;
-          yk[q][4] = b.x; yk[q][5] = b.y; yk[q][6] = b.z; yk[q][7] = b.w;
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int r = r0 + q;
-        if (r < k && rows[r] >= 0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i] = __fadd_rn(acc[i], fp32 ? yk[q][i] : round_dt<DT>(yk[q][i]));
-        }
-      }
-    }
-    const float4* src = reinterpret_cast<const float4*>(p.y_shared + (size_t)t * H + h);
-    const float4 a = src[0], b = src[1];
-    const float s[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    uint4 o;
-    uint16_t* os = reinterpret_cast<uint16_t*>(&o);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float v = fp32 ? __fadd_rn(acc[i], s[i]) : __fadd_rn(round_dt<DT>(acc[i]), round_dt<DT>(s[i]));
-      os[i] = Half16<DT>::from_f(v);
-    }
-    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + (size_t)t * H + h) = o;
-  }
-  if (p.tl && threadIdx.x == 0) tl_max(p.tl + 2);
-}
-
 static cudaError_t launch_shared_gate(const CombineParams& p, cudaStream_t st);
+
+template <int DT>
+static cudaError_t launch_combine_rule(int rule, dim3 grid, bool early, const CombineParams& p, cudaStream_t st) {
+  void (*kernel)(const CombineParams) = rule == RULE_LLAMA4 ? combine_kernel<DT, RULE_LLAMA4>
+                                        : rule == RULE_QWEN ? combine_kernel<DT, RULE_QWEN>
+                                                            : combine_kernel<DT, RULE_PLAIN>;
+  return launch_cluster(kernel, grid, dim3(CB_THREADS), 0, st, 1, early, p);
+}
 
 cudaError_t launch_combine(const CombineParams& p, cudaStream_t st) {
   if (p.T == 0) return cudaSuccess;
@@ -1532,22 +1471,15 @@ cudaError_t launch_combine(const CombineParams& p, cudaStream_t st) {
   int gy = (p.H + CB_THREADS * 8 - 1) / (CB_THREADS * 8);
   dim3 grid(p.T, gy);
   if (p.dtype == DT_F32) return launch_combine_f32(p, st);
-  if (p.unweighted || p.mode == COMBINE_LLAMA4) {
-    if (!p.unweighted || (p.mode != COMBINE_LLAMA4 && p.mode != COMBINE_FP32) || !p.y_shared || p.ep_collect || p.shared_gate)
-      return cudaErrorInvalidValue;
-    if (p.dtype == DT_BF16) return launch_cluster(combine_llama4_kernel<DT_BF16>, grid, dim3(CB_THREADS), 0, st, 1, false, p);
-    if (p.dtype == DT_F16) return launch_cluster(combine_llama4_kernel<DT_F16>, grid, dim3(CB_THREADS), 0, st, 1, false, p);
+  const int rule = (p.unweighted || p.mode == COMBINE_LLAMA4) ? RULE_LLAMA4
+                   : (p.mode == COMBINE_QWEN || p.shared_gate) ? RULE_QWEN : RULE_PLAIN;
+  if (rule == RULE_LLAMA4 && (!p.unweighted || (p.mode != COMBINE_LLAMA4 && p.mode != COMBINE_FP32) || !p.y_shared ||
+                              p.ep_collect || p.shared_gate))
     return cudaErrorInvalidValue;
-  }
-  const bool early = p.ep_collect && p.ep.direct && p.ep_early;
-  const bool qwen = p.mode == COMBINE_QWEN || p.shared_gate;
-  if (qwen && (p.ep_collect || (p.y_shared && !p.shared_gate))) return cudaErrorInvalidValue;
-  if (p.dtype == DT_BF16)
-    return qwen ? launch_cluster(combine_kernel<DT_BF16, true>, grid, dim3(CB_THREADS), 0, st, 1, false, p)
-                : launch_cluster(combine_kernel<DT_BF16, false>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
-  if (p.dtype == DT_F16)
-    return qwen ? launch_cluster(combine_kernel<DT_F16, true>, grid, dim3(CB_THREADS), 0, st, 1, false, p)
-                : launch_cluster(combine_kernel<DT_F16, false>, grid, dim3(CB_THREADS), 0, st, 1, early, p);
+  if (rule == RULE_QWEN && (p.ep_collect || (p.y_shared && !p.shared_gate))) return cudaErrorInvalidValue;
+  const bool early = rule == RULE_PLAIN && p.ep_collect && p.ep.direct && p.ep_early;
+  if (p.dtype == DT_BF16) return launch_combine_rule<DT_BF16>(rule, grid, early, p, st);
+  if (p.dtype == DT_F16) return launch_combine_rule<DT_F16>(rule, grid, early, p, st);
   return cudaErrorInvalidValue;
 }
 
