@@ -385,6 +385,10 @@ int b2m_last_lookahead(b2m_ctx* ctx, int32_t* look_host);
  *   Passing NULL for send_counts / recv_counts selects the inline layout: all four row buffers are
  *   [nranks][cap+1][H] and the extra last row of every peer segment carries counts[E] (int32, needs 4E <= 2H),
  *   so one all-to-all moves rows and counts together.
+ * A context with B2M_NUMERICS_FP32 is refused with B2M_EUNSUPPORTED by these four and by b2m_ep_p2p_init (so the
+ * peer-to-peer calls below never run on it): the rows come back in the model dtype, so each expert output would be rounded
+ * once more than on one GPU, where the fp32 combine reads it unrounded, and the result would depend on the exchange mode
+ * (the peer-to-peer direct mode reads the owners' fp32 outputs in place).
  * Call order per layer: b2m_route -> b2m_ep_pack -> (exchange counts+rows) -> b2m_ep_regroup -> b2m_run_experts(T_total)
  *   -> b2m_ep_ungroup -> (exchange back) -> b2m_ep_unpack -> b2m_combine. */
 int b2m_ep_pack(b2m_ctx* ctx, int nranks, int rank, int cap, int T_local, void* send_rows, int32_t* send_counts,

@@ -1275,7 +1275,8 @@ static int route_impl(b2m_ctx* c, int layer, const void* x, const void* router_i
       return fail(c, B2M_EUNSUPPORTED, "fp32 contexts take router logits / scores (or a mask): the fused gate kernel reads 16-bit activations");
     if (!p.gate_w) return fail(c, B2M_ESTATE, "layer %d has no gate weight (b2m_set_gate) and no router input", layer);
   } else {
-    if (!router_in) return fail(c, B2M_EINVAL, "router_in is null");
+    // no tokens, nothing to read: an expert-parallel rank with an empty batch hands over an empty (null) router input
+    if (!router_in && T > 0) return fail(c, B2M_EINVAL, "router_in is null");
     p.logits = router_in;
     p.logits_dtype = in_dtype;
     p.logits_are_scores = (kind == 2);
@@ -1944,6 +1945,11 @@ static EpParams ep_base(b2m_ctx* c, int nranks, int rank, int cap) {
 static int ep_check(b2m_ctx* c, int nranks, int rank, int cap) {
   if (!c) return B2M_EINVAL;
   if (c->cfg.dtype == B2M_DTYPE_F32) return fail(c, B2M_EUNSUPPORTED, "expert parallel exchange handles 16-bit models");
+  // the buffer exchange returns expert outputs in the model dtype, the single-GPU fp32 combine reads them unrounded (and
+  // the peer-to-peer direct mode reads the owners' fp32 outputs): the result would depend on the exchange mode
+  if (c->cfg.numerics == B2M_NUMERICS_FP32)
+    return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with fp32 numerics (B2M_NUMERICS_FP32): the "
+                "exchange returns expert outputs rounded to the model dtype");
   if (c->wf->a_src != AS_BF16) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with %s weights", c->wf->name);
   if (!c->rk->ep) return fail(c, B2M_EUNSUPPORTED, "expert parallelism is not available with the %s router", c->rk->name);
   if (nranks < 2 || nranks > 16 || rank < 0 || rank >= nranks || c->cfg.num_experts % nranks || cap < 1)
