@@ -259,6 +259,21 @@ int b2m_ctx_destroy(b2m_ctx* ctx);
                                        B2M_EUNSUPPORTED and a message: cfg.dtype f16; expert types Mixtral (4) and DeepSeek
                                        (5); hidden and inter multiples of 128; gemm_impl 0 or 2.  The expert-parallel entry
                                        points return B2M_EUNSUPPORTED on such a context. */
+#define B2M_WEIGHTS_FP8_E4M3_ROW 7  /* FP8 E4M3 matrices with one fp32 scale per output channel (Llama 4 Maverick FP8 and other
+                                       fbgemm FP8 checkpoints; a per-tensor scale is this format with the scalar repeated).
+                                       Each routed matrix (nn.Linear [out,in], row-major) is float8_e4m3fn with an fp32 scale
+                                       vector s[out]; the scale multiplies.  The experts compute exactly what the bf16 engine
+                                       computes on
+                                         W[r][c] = bf16(fp32(w_q[r][c]) * s[r])
+                                       -- one fp32 multiply rounded to nearest-even, then one rounding to bf16 (torch:
+                                       `(w_q.float() * s[:, None]).to(torch.bfloat16)`); the GEMMs dequantise inside the
+                                       kernel, so results are bit-identical to a bf16 context holding those W.
+                                       Expert blob, 3*H*I + 4*(2*I + H) bytes rounded up to a multiple of 16: the three e4m3
+                                       matrices in the model's tensor order (Mixtral w1|w2|w3, DeepSeek gate|up|down), then
+                                       their three scale vectors in the same order (lengths I, H, I for Mixtral; I, I, H for
+                                       gate|up|down), zero-padded.  Activations, outputs, workspaces, the router and the shared
+                                       experts stay bf16.  Restrictions (B2M_EUNSUPPORTED with a message) and the
+                                       expert-parallel refusal: as B2M_WEIGHTS_FP8_E4M3_B128. */
 /* b2m_ctx_create with the routed experts stored in `weight_format` (B2M_WEIGHTS_*; any other value: B2M_EINVAL) */
 int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out);
 /* B2M_WEIGHTS_INT4_G128_F16 only: act-order GPTQ (desc_act).  `dev_perm` is a borrowed device table uint16 [E][H] (like the

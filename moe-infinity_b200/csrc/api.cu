@@ -89,13 +89,15 @@ struct WeightFormat {
   const char* name;                     // in messages
   int act_dtype;                        // the model dtype (activations) the format needs; -1 = any
   int bits;                             // bits per stored weight; 0 = the model dtype's
-  size_t (*grid_bytes)(int H, int I);   // bytes of one matrix's side grid (block scales / group words); null = none
+  size_t (*grid_bytes)(int rows, int cols);   // bytes of the side grid (block scales / row scales / group words) of a
+                                              // rows x cols matrix; null = none
   int hi_multiple;                      // hidden and inter must be multiples of this
   int a_src;                            // AS_*: how the tensor-core GEMMs read the weights
 };
 const WeightFormat WEIGHT_FORMATS[] = {
     {B2M_WEIGHTS_MODEL_DTYPE, "model-dtype", -1, 0, nullptr, 1, AS_BF16},
     {B2M_WEIGHTS_FP8_E4M3_B128, "fp8", B2M_DTYPE_BF16, 8, f8::scale_grid_bytes, f8::BLOCK, AS_FP8},
+    {B2M_WEIGHTS_FP8_E4M3_ROW, "fp8 (row scales)", B2M_DTYPE_BF16, 8, f8::row_scale_bytes, f8::BLOCK, AS_FP8_ROW},
     {B2M_WEIGHTS_INT4_G128, "int4", B2M_DTYPE_BF16, 4, i4::grid_bytes, i4::GROUP, AS_INT4},
     {B2M_WEIGHTS_INT4_G128_F16, "int4 (fp16 scales)", B2M_DTYPE_F16, 4, i4::grid_bytes, i4::GROUP, AS_INT4},
 };
@@ -337,9 +339,10 @@ int fail(b2m_ctx* c, int code, const char* fmt, ...) {
   } while (0)
 
 // Slot layout of one expert: its matrices in the model's tensor order, H * I * bits / 8 bytes each, then (quantised formats)
-// one side grid of grid_bytes per matrix in the same order; rounded up to 16 B so that TMA strides stay multiples of 16 B.
-// For fp8 and int4 this is f8::expert_blob_bytes / i4::expert_blob_bytes.
-bool make_shape(int expert_type, int H, int I, int bits, size_t grid_bytes, ExpertShape* s) {
+// the side grid of each matrix, grid_bytes(rows, cols), in the same order; rounded up to 16 B so that TMA strides stay
+// multiples of 16 B.  For the quantised formats this is f8::expert_blob_bytes, f8::row_expert_blob_bytes and
+// i4::expert_blob_bytes.
+bool make_shape(int expert_type, int H, int I, int bits, size_t (*grid_bytes)(int, int), ExpertShape* s) {
   const size_t m = (size_t)H * I * bits / 8, esize = bits / 8;
   s->H = H;
   s->I = I;
@@ -367,10 +370,18 @@ bool make_shape(int expert_type, int H, int I, int bits, size_t grid_bytes, Expe
       return false;
   }
   if (grid_bytes) {
-    s->grid_gate = 3 * m + s->off_gate / m * grid_bytes;
-    s->grid_up = 3 * m + s->off_up / m * grid_bytes;
-    s->grid_down = 3 * m + s->off_down / m * grid_bytes;
-    s->bytes += 3 * grid_bytes;
+    // matrix j of the blob starts at j * m; the grids follow the matrices in that order (gate / up [I x H], down [H x I])
+    const size_t g_in = grid_bytes(I, H), g_dn = grid_bytes(H, I);
+    const size_t j_dn = s->off_down / m;
+    auto grid_of = [&](size_t off) {
+      size_t o = 3 * m;
+      for (size_t j = 0; j < off / m; ++j) o += j == j_dn ? g_dn : g_in;
+      return o;
+    };
+    s->grid_gate = grid_of(s->off_gate);
+    s->grid_up = grid_of(s->off_up);
+    s->grid_down = grid_of(s->off_down);
+    s->bytes += 2 * g_in + g_dn;
   }
   s->bytes = (s->bytes + 15) & ~(size_t)15;
   return true;
@@ -832,8 +843,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
       cfg->max_tokens < 1)
     return fail(nullptr, B2M_EINVAL, "bad model dimensions");
   ExpertShape shape;
-  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, wf->bits ? wf->bits : 8 * (int)esize,
-                  wf->grid_bytes ? wf->grid_bytes(cfg->hidden, cfg->inter) : 0, &shape))
+  if (!make_shape(cfg->expert_type, cfg->hidden, cfg->inter, wf->bits ? wf->bits : 8 * (int)esize, wf->grid_bytes, &shape))
     return fail(nullptr, B2M_EUNSUPPORTED, "expert_type %d is unknown (expert_module.h:13-18 defines 0..5)", cfg->expert_type);
   if (wf->a_src != AS_BF16) {   // a quantised format: three matrices per expert, decoded inside the tensor-core GEMMs
     if (cfg->dtype != wf->act_dtype)
@@ -951,7 +961,7 @@ int b2m_ctx_create_ex(const b2m_config* cfg, int weight_format, b2m_ctx** out) {
   if (r) { g_create_error = c->err; b2m_ctx_destroy(c); return r; }
   if (cfg->shared_inter > 0) {
     ExpertShape ss;
-    make_shape(B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, H, cfg->shared_inter, 8 * (int)esize, 0, &ss);
+    make_shape(B2M_EXPERT_DEEPSEEK_MOE_DENSE_ACT_DENSE, H, cfg->shared_inter, 8 * (int)esize, nullptr, &ss);
     c->shared_arena.shape = ss;
     c->shared_arena.slot_bytes = ss.bytes;
     c->shared_arena.nslots = L;

@@ -36,7 +36,8 @@ enum : int {
 enum : int { AS_BF16 = 0,   // bf16 tile in shared memory, read by the wgmma itself
              AS_PK12 = 1,   // bf16 tile or 12-bit packed record (weight_pack.cuh), decoded into register fragments
              AS_FP8 = 2,    // e4m3 tile + 128x128 block scales (fp8_weights.cuh), dequantised into register fragments
-             AS_INT4 = 3 }; // 4-bit code tile + per-128-input scale / zero point (int4_weights.cuh), dequantised likewise
+             AS_INT4 = 3,   // 4-bit code tile + per-128-input scale / zero point (int4_weights.cuh), dequantised likewise
+             AS_FP8_ROW = 4 };  // e4m3 tile as AS_FP8 + one fp32 scale per weight row (fp8_weights.cuh)
 
 struct GemmParams {
   const int* offsets;   // [E+1] first permuted row of each expert
@@ -102,9 +103,9 @@ struct GemmParams {
   int pack_rows[3], pack_cols[3];
   uint8_t* pack_dst;         // packed arena (pk_slot_bytes per slot)
   int* pack_ok;              // = pk_ok, writable
-  // ---- quantised weights (AS_FP8, AS_INT4): the A maps are uint8 maps over the quantised matrices, and grid0 / grid1 are
-  // the side grids of A0 / A1 in slot 0, grid_slot_bytes apart: fp32 block scales [M / 128][K / 128] (fp8_weights.cuh) or
-  // tile-major group words, one uint32 per row and 128 k (int4_weights.cuh)
+  // ---- quantised weights (AS_FP8, AS_FP8_ROW, AS_INT4): the A maps are uint8 maps over the quantised matrices, and grid0 / grid1 are
+  // the side grids of A0 / A1 in slot 0, grid_slot_bytes apart: fp32 block scales [M / 128][K / 128] or row scales [M]
+  // (fp8_weights.cuh), or tile-major group words, one uint32 per row and 128 k (int4_weights.cuh)
   const uint8_t* grid0;
   const uint8_t* grid1;
   size_t grid_slot_bytes;

@@ -1,4 +1,5 @@
-// fp8_weights.cuh -- routed experts stored as FP8 E4M3 with one fp32 scale per 128 x 128 block (B2M_WEIGHTS_FP8_E4M3_B128).
+// fp8_weights.cuh -- routed experts stored as FP8 E4M3 with one fp32 scale per 128 x 128 block (B2M_WEIGHTS_FP8_E4M3_B128)
+// or one fp32 scale per output channel, i.e. per matrix row (B2M_WEIGHTS_FP8_E4M3_ROW).
 //
 // Semantics (include/b2m.h): the experts compute exactly what the bf16 engine computes on
 //   W[r][c] = bf16(fp32(w_q[r][c]) * s[r / 128][c / 128])
@@ -11,6 +12,9 @@
 // Expert blob in a slot: the three e4m3 matrices in the model's tensor order (Mixtral w1 | w2 | w3, DeepSeek gate | up |
 // down), then their three fp32 scale grids [rows / 128][cols / 128] in the same order, zero-padded to a multiple of 16 B so
 // that TMA global strides stay multiples of 16 B.
+// Row format: the same, with s[r][c] = s[r] and scale vectors s[rows] in place of the grids (lengths I, H, I for Mixtral;
+// I, I, H for gate | up | down).  A consumer thread's A fragments cover two rows of the tile (ra and ra + 8), so it loads
+// their two scales once per tile and decodes every k-block with them (decode_lane's two-scale form).
 //
 // GEMM A tile: 128 rows x 64 k = 64-byte rows, 8 KiB, loaded by TMA (uint8 elements) with SWIZZLE_64B: byte (row, col) sits
 // at row * 64 + ((col >> 4) ^ ((row >> 1) & 3)) * 16 + (col & 15).  A consumer thread reads the two bytes of each register
@@ -51,6 +55,13 @@ F8_HD size_t scale_grid_offset(int H, int I, size_t mat_off) {
   const size_t m = (size_t)H * (size_t)I;
   return 3 * m + (mat_off / m) * scale_grid_bytes(H, I);
 }
+// row format: one fp32 scale per row of a rows x cols matrix
+F8_HD size_t row_scale_bytes(int rows, int cols) { return (size_t)rows * 4; }
+// an expert of two [I x H] matrices and one [H x I]: 3 e4m3 matrices + scale vectors of I, I and H rows, rounded up to 16 B
+F8_HD size_t row_expert_blob_bytes(int H, int I) {
+  const size_t b = 3 * (size_t)H * (size_t)I + 2 * row_scale_bytes(I, H) + row_scale_bytes(H, I);
+  return (b + 15) & ~(size_t)15;
+}
 
 // ---- per-element decode (host and device; the device GEMM path below does the same arithmetic two values at a time)
 // e4m3fn code -> its exact fp32 value (exponent bias 7, no infinities, S.1111.111 = NaN)
@@ -76,6 +87,11 @@ F8_HD uint16_t float_to_bf16_rn(float f) {
 }
 // the dequantised bf16 bits of code c under scale s
 F8_HD uint16_t dequant(uint8_t c, float s) { return float_to_bf16_rn(e4m3_to_float(c) * s); }
+// row format: the dequantised bf16 bits of a row-major rows x cols e4m3 matrix q under its row scales s[rows]
+inline void dequant_rows(const uint8_t* q, const float* s, int rows, int cols, uint16_t* w) {
+  for (int r = 0; r < rows; ++r)
+    for (int c = 0; c < cols; ++c) w[(size_t)r * cols + c] = dequant(q[(size_t)r * cols + c], s[r]);
+}
 
 // byte offset of (row, col) inside a SWIZZLE_64B A tile
 F8_HD uint32_t tile_offset(int row, int col) {
@@ -95,8 +111,9 @@ __device__ __forceinline__ uint32_t dequant2(uint16_t codes, float s) {
   return d;
 }
 // lane L's A fragments of one k-block (m64k16 layout of weight_pack.cuh's lane_coord: a[4j + r] = register r of k16 step j,
-// r & 1 -> row + 8, r & 2 -> k + 8) from a SWIZZLE_64B e4m3 tile in shared memory, dequantised with scale s
-__device__ __forceinline__ void decode_lane(const uint8_t* tile, int L, float s, uint32_t (&a)[16]) {
+// r & 1 -> row + 8, r & 2 -> k + 8) from a SWIZZLE_64B e4m3 tile in shared memory, dequantised with scale s0 in row r0 and
+// s1 in row r0 + 8 (row format: the two rows' scales; block format: s0 == s1, the block's scale)
+__device__ __forceinline__ void decode_lane(const uint8_t* tile, int L, float s0, float s1, uint32_t (&a)[16]) {
   const int t = L & 127, g = (t & 31) >> 2, tig = t & 3;
   const int r0 = (L >> 7) * 64 + (t >> 5) * 16 + g;                 // rows r0, r0 + 8 share (row >> 1) & 3
   const uint32_t sw = (uint32_t)((r0 >> 1) & 3);
@@ -112,11 +129,13 @@ __device__ __forceinline__ void decode_lane(const uint8_t* tile, int L, float s,
       const uint32_t w_hi = *reinterpret_cast<const uint32_t*>(p + 8);   // k 16j + 8..15
       uint32_t q;
       asm("prmt.b32 %0, %1, %2, %3;" : "=r"(q) : "r"(w_lo), "r"(w_hi), "r"(sel));
+      const float s = h ? s1 : s0;
       a[4 * j + h] = dequant2((uint16_t)(q & 0xffff), s);
       a[4 * j + 2 + h] = dequant2((uint16_t)(q >> 16), s);
     }
   }
 }
+__device__ __forceinline__ void decode_lane(const uint8_t* tile, int L, float s, uint32_t (&a)[16]) { decode_lane(tile, L, s, s, a); }
 #endif
 
 }  // namespace f8

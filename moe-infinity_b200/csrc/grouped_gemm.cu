@@ -40,7 +40,7 @@ constexpr int SMEM_BUDGET = 216 * 1024;   // of the 227 KiB a block may use on s
 
 template <int NT, bool DUAL, int AS = AS_BF16>
 struct GemmCfg {
-  static constexpr int A_BYTES = AS == AS_FP8 ? f8::TILE_BYTES : AS == AS_INT4 ? i4::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
+  static constexpr int A_BYTES = (AS == AS_FP8 || AS == AS_FP8_ROW) ? f8::TILE_BYTES : AS == AS_INT4 ? i4::TILE_BYTES : A_TILE_BYTES;   // one A tile of a stage
   static constexpr int B_TILE_BYTES = NT * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = (DUAL ? 2 : 1) * A_BYTES + B_TILE_BYTES;
   static constexpr int STAGES_RAW = SMEM_BUDGET / STAGE_BYTES;
@@ -128,6 +128,8 @@ __device__ __forceinline__ void grid_bar_wait(const GridBar& g) {
 // FP8 (AS_FP8: bf16, MC == 1, no m_rows / expert-parallel regions; every tile width): the A maps are uint8 maps over e4m3
 // matrices; the producer loads 8-KiB e4m3 tiles and the consumers dequantise their fragments with the tile's block scale
 // (fp8_weights.cuh) into the same register-A wgmmas, over the same tile walk and launch plan as the bf16 engine.
+// FP8_ROW (AS_FP8_ROW: as FP8, with one scale per weight row): each consumer thread loads the scales of its two rows once per
+// tile and dequantises every k-block with them.
 // INT4 (AS_INT4: same restrictions and plan as FP8, but bf16 or f16 -- the group scales are of the activations' type): the A
 // maps are uint8 maps over the 4-bit code matrices (32-byte rows); the producer loads 4-KiB code tiles and the consumers
 // dequantise their fragments with the group words of their rows (int4_weights.cuh), read from the tile-major group grids
@@ -136,7 +138,7 @@ template <int NT, bool DUAL, int DT, int MC, bool REGSPLIT = true, int AS = AS_B
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
                                           const GemmParams& p, uint8_t* smem, int dep_mode, const GridBar& gbar, int ctas) {
   using Cfg = GemmCfg<NT, DUAL, AS>;
-  constexpr bool PK = AS == AS_PK12, F8 = AS == AS_FP8, I4 = AS == AS_INT4;
+  constexpr bool PK = AS == AS_PK12, F8 = AS == AS_FP8 || AS == AS_FP8_ROW, F8R = AS == AS_FP8_ROW, I4 = AS == AS_INT4;
   constexpr int A_BYTES = Cfg::A_BYTES;
   // carve shared memory: [stages | barriers | tile tables]
   uint8_t* stage_base = smem;
@@ -389,7 +391,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
       const float* sc0 = nullptr;
       const float* sc1 = nullptr;
       float sn0 = 0.f, sn1 = 0.f;
-      if constexpr (F8) {
+      if constexpr (F8 && !F8R) {
         const int kbs = p.K / f8::BLOCK, mt = t.m0 / BLOCK_M, mts = p.M / BLOCK_M;
         sc0 = reinterpret_cast<const float*>(p.grid0 + (size_t)t.slot * p.grid_slot_bytes) + (size_t)mt * kbs;
         sc1 = DUAL ? reinterpret_cast<const float*>(p.grid1 + (size_t)t.slot * p.grid_slot_bytes) +
@@ -423,11 +425,24 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
                         : grp.w[0];
         grp.load(t.kb_begin);
       }
+      // FP8_ROW: scales of this thread's rows ra, ra + 8 in A0 / A1 (dual_m as for FP8; a row past the matrix -- TMA zero fill,
+      // dropped in the epilogue -- gets 0), loaded once per tile
+      float rs[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+      if constexpr (F8R) {
+        const float* r0 = reinterpret_cast<const float*>(p.grid0 + (size_t)t.slot * p.grid_slot_bytes);
+        const float* r1 = reinterpret_cast<const float*>(p.grid1 + (size_t)t.slot * p.grid_slot_bytes);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = t.m0 + ra + 8 * h, m1 = m + (p.dual_m ? BLOCK_M : 0);
+          rs[0][h] = m < p.M ? __ldg(r0 + m) : 0.f;
+          if (DUAL) rs[1][h] = m1 < p.M ? __ldg(r1 + m1) : 0.f;
+        }
+      }
       // one k-block, A decoded from packed records / dequantised from e4m3 into fragment buffer BUF (compile time)
       auto kblock_packed = [&](int kb, auto BUF) {
         constexpr int bf = decltype(BUF)::value;
         float s0 = 0.f, s1 = 0.f;
-        if constexpr (F8) {
+        if constexpr (F8 && !F8R) {
           s0 = sn0;
           s1 = sn1;
           if (kb + 1 < t.kb_end) {
@@ -443,7 +458,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA0, const CUtenso
         mbar_wait(&full_bar[stage], phase);
         if constexpr (FRAG_BUFS == 1) wgmma_wait<0>();   // the previous k-block's wgmmas have read the fragments
         const uint8_t* sa = stage_base + stage * Cfg::STAGE_BYTES;
-        if constexpr (F8) {
+        if constexpr (F8R) {
+          f8::decode_lane(sa, ct, rs[0][0], rs[0][1], fa0[bf]);
+          if constexpr (DUAL) f8::decode_lane(sa + A_BYTES, ct, rs[1][0], rs[1][1], fa1[bf]);
+        } else if constexpr (F8) {
           f8::decode_lane(sa, ct, s0, fa0[bf]);
           if constexpr (DUAL) f8::decode_lane(sa + A_BYTES, ct, s1, fa1[bf]);
         } else if constexpr (I4) {
@@ -574,10 +592,8 @@ __device__ __forceinline__ uint8_t* smem_aligned(uint8_t* raw) {
 }
 
 template <int NT, bool DUAL, int DT, int MC, int AS>
-__global__ void __launch_bounds__((GemmCfg<NT, DUAL, AS>::THREADS), 1)
-grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                       const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
+__device__ __forceinline__ void tc_kernel_body(const CUtensorMap& tmA0, const CUtensorMap& tmA1, const CUtensorMap& tmB,
+                                               const GemmParams& p, uint8_t* smem_raw) {
   uint8_t* smem = smem_aligned(smem_raw);
   if (p.tl && threadIdx.x == 0) tl_min(p.tl);
   // pdl_edge: this grid may be resident long before its predecessor finishes (expert parallel: the gate/up GEMM arrives behind the
@@ -587,6 +603,24 @@ grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_co
   GridBar nobar{nullptr, 0};
   gemm_body<NT, DUAL, DT, MC, true, AS>(tmA0, tmA1, tmB, p, smem, DEP_PDL, nobar, (int)gridDim.x);
   gemm_finish<MC>(p);
+}
+
+template <int NT, bool DUAL, int DT, int MC, int AS>
+__global__ void __launch_bounds__((GemmCfg<NT, DUAL, AS>::THREADS), 1)
+grouped_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                       const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  tc_kernel_body<NT, DUAL, DT, MC, AS>(tmA0, tmA1, tmB, p, smem_raw);
+}
+
+// The same GEMM for row-scaled fp8 experts (AS_FP8_ROW: bf16, MC == 1) under a name of its own, so that profiles and the
+// library's SASS tell the two fp8 formats' kernels apart.
+template <int NT, bool DUAL>
+__global__ void __launch_bounds__((GemmCfg<NT, DUAL, AS_FP8_ROW>::THREADS), 1)
+grouped_gemm_fp8_row_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                            const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  tc_kernel_body<NT, DUAL, DT_BF16, 1, AS_FP8_ROW>(tmA0, tmA1, tmB, p, smem_raw);
 }
 
 #ifdef B2M_ENABLE_FUSED_FFN
@@ -694,11 +728,21 @@ __global__ void grouped_gemm_simt_kernel(const uint16_t* __restrict__ arena, siz
 // --------------------------------------------------------------------------------------
 // host launchers
 // --------------------------------------------------------------------------------------
+template <int NT, bool DUAL, int DT, int MC, int AS>
+static auto tc_kernel() {
+  if constexpr (AS == AS_FP8_ROW) {
+    static_assert(DT == DT_BF16 && MC == 1, "row-scaled fp8 weights: bf16 activations, single-CTA tiles");
+    return grouped_gemm_fp8_row_kernel<NT, DUAL>;
+  } else {
+    return grouped_gemm_tc_kernel<NT, DUAL, DT, MC, AS>;
+  }
+}
+
 template <int NT, bool DUAL, int DT, int MC = 1, int AS = AS_BF16>
 static cudaError_t launch_tc(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmParams& p,
                              int grid, cudaStream_t st) {
   using Cfg = GemmCfg<NT, DUAL, AS>;
-  auto kern = grouped_gemm_tc_kernel<NT, DUAL, DT, MC, AS>;
+  auto kern = tc_kernel<NT, DUAL, DT, MC, AS>();
   static bool attr_done = false;   // per-instantiation
   if (!attr_done) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -934,6 +978,7 @@ cudaError_t launch_grouped_gemm_tc(int dtype, int nt, bool dual, const CUtensorM
       case AS_BF16: return pk ? launch_nt<DT_BF16, AS_PK12>(nt, dual, a0, a1, b, p, grid, st)
                               : launch_nt<DT_BF16, AS_BF16>(nt, dual, a0, a1, b, p, grid, st);
       case AS_FP8: return launch_nt<DT_BF16, AS_FP8>(nt, dual, a0, a1, b, p, grid, st);
+      case AS_FP8_ROW: return launch_nt<DT_BF16, AS_FP8_ROW>(nt, dual, a0, a1, b, p, grid, st);
       case AS_INT4: return launch_nt<DT_BF16, AS_INT4>(nt, dual, a0, a1, b, p, grid, st);
     }
   } else if (dtype == DT_F16) {   // (no packed copy, no fp8 weights)

@@ -21,6 +21,7 @@ NUMERICS_REFERENCE, NUMERICS_FP32 = 0, 1
 CACHE_REFERENCE, CACHE_SLOTS, CACHE_ACTIVATION_AWARE = 0, 1, 2
 WEIGHTS_MODEL_DTYPE, WEIGHTS_FP8_E4M3_B128 = 0, 1
 WEIGHTS_INT4_G128, WEIGHTS_INT4_G128_F16 = 4, 6
+WEIGHTS_FP8_E4M3_ROW = 7
 WS = dict(topk_idx=0, topk_w=1, row_of=2, perm_token=3, counts=4, offsets=5, xp=6, hmid=7, y=8, scores=9, logits=10,
           shared_gate=11, y_shared=12)
 

@@ -52,13 +52,16 @@ class MoEEngine:
                  expert_capacity: int = 0, gate_dtype: Optional[torch.dtype] = None, device: int = 0,
                  max_inflight_prefetch: int = 2, h2d_chunk_bytes: int = 0, gemm_impl: int = 0,
                  cache_policy: int = L.CACHE_REFERENCE, lookahead_prefetch: bool = False, freq_alpha: float = 0.0,
-                 pack_weights: bool = True, expert_dtype: Optional[torch.dtype] = None):
+                 pack_weights: bool = True, expert_dtype: Optional[torch.dtype] = None, fp8_scales: str = "block128"):
         """expert_dtype: None = the routed experts are stored in `dtype`; torch.float8_e4m3fn = FP8 E4M3 with one fp32 scale
         per 128x128 block (`fp8.py`; `dtype` stays the activation dtype and must be bf16; register_expert / load_expert then
         take the three e4m3 matrices and their scale grids); torch.uint4 = 4-bit codes with a 16-bit scale and a 4-bit zero
         point per 128 inputs (`int4.py`; register_expert / load_expert then take the three packed code matrices with scales=
         and zeros=).  The scales are of `dtype`: bf16 (B2M_WEIGHTS_INT4_G128) or float16 (B2M_WEIGHTS_INT4_G128_F16, the
-        AWQ / GPTQ format: `int4.from_awq`, `int4.from_gptq`, `hf.load_int4_checkpoint`)."""
+        AWQ / GPTQ format: `int4.from_awq`, `int4.from_gptq`, `hf.load_int4_checkpoint`).
+        fp8_scales (fp8 engines): "block128" (the default, above) or "row": one fp32 scale per output channel
+        (B2M_WEIGHTS_FP8_E4M3_ROW, `fp8.dequantize_row`; the fbgemm FP8 format, `hf.load_fp8_checkpoint`); the scales
+        given to register_expert / load_expert are then float32 [out] (or [out, 1]) vectors."""
         self.lib = L.load()
         if not torch.cuda.is_available():
             raise RuntimeError("moe_infinity_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -67,6 +70,11 @@ class MoEEngine:
         if expert_dtype is not None and expert_dtype not in (torch.float8_e4m3fn, torch.uint4):
             raise ValueError(f"unsupported expert_dtype {expert_dtype} (None, torch.float8_e4m3fn or torch.uint4)")
         self.fp8 = expert_dtype == torch.float8_e4m3fn
+        if fp8_scales not in ("block128", "row"):
+            raise ValueError(f"fp8_scales {fp8_scales!r}: 'block128' or 'row'")
+        if fp8_scales != "block128" and not self.fp8:
+            raise ValueError("fp8_scales goes with an fp8 engine (expert_dtype=torch.float8_e4m3fn)")
+        self.fp8_scales = fp8_scales if self.fp8 else None
         self.int4 = expert_dtype == torch.uint4
         if self.fp8 and dtype != torch.bfloat16:
             raise ValueError("fp8 experts compute with bf16 activations: dtype must be torch.bfloat16")
@@ -106,7 +114,7 @@ class MoEEngine:
         torch.cuda.set_device(self.device)
         fmt = L.WEIGHTS_MODEL_DTYPE
         if self.fp8:
-            fmt = L.WEIGHTS_FP8_E4M3_B128
+            fmt = L.WEIGHTS_FP8_E4M3_ROW if fp8_scales == "row" else L.WEIGHTS_FP8_E4M3_B128
         elif self.int4:
             fmt = L.WEIGHTS_INT4_G128_F16 if dtype == torch.float16 else L.WEIGHTS_INT4_G128
         L.check(None, self.lib.b2m_ctx_create_ex(C.byref(cfg), fmt, C.byref(h)))
@@ -151,7 +159,8 @@ class MoEEngine:
         return blob
 
     def _fp8_parts(self, tensors: Sequence[torch.Tensor], scales: Optional[Sequence[torch.Tensor]]) -> List[torch.Tensor]:
-        """The fp8 expert blob's parts as flat uint8 tensors: three e4m3 matrices, then their fp32 scale grids."""
+        """The fp8 expert blob's parts as flat uint8 tensors: three e4m3 matrices, then their fp32 scale grids (row scales:
+        vectors)."""
         if scales is None:
             raise ValueError("an fp8 engine needs the three scale grids: scales=(s1, s2, s3)")
         if len(tensors) != 3 or len(scales) != 3:
@@ -165,6 +174,12 @@ class MoEEngine:
                 raise ValueError(f"expected a float8_e4m3fn {shp} matrix, got {t.dtype} {tuple(t.shape)}")
             parts.append(t.detach().contiguous().view(torch.uint8).reshape(-1))
         for s, shp in zip(scales, shapes):
+            if self.fp8_scales == "row":
+                if s.dtype != torch.float32 or tuple(s.shape) not in ((shp[0],), (shp[0], 1)):
+                    raise ValueError(f"expected a float32 ({shp[0]},) or ({shp[0]}, 1) row-scale vector, got {s.dtype} "
+                                     f"{tuple(s.shape)}")
+                parts.append(s.detach().contiguous().view(torch.uint8).reshape(-1))
+                continue
             want = (shp[0] // F8.BLOCK, shp[1] // F8.BLOCK)
             if s.dtype != torch.float32 or tuple(s.shape) != want:
                 raise ValueError(f"expected a float32 {want} scale grid, got {s.dtype} {tuple(s.shape)}")
@@ -211,7 +226,8 @@ class MoEEngine:
                         scales: Optional[Sequence[torch.Tensor]] = None, zeros: Optional[Sequence[torch.Tensor]] = None):
         """Host-backed expert (can be staged in and evicted).  tensors: Mixtral (w1,w2,w3),
         DeepSeek (gate,up,down), Switch (wi,wo), NLLB/FSGPT (fc1,fc1_bias,fc2,fc2_bias) -- nn.Linear [out,in] layout.
-        fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids.
+        fp8 engine: the three float8_e4m3fn matrices and `scales`, their float32 [out/128, in/128] grids (fp8_scales="row":
+        float32 [out] vectors).
         int4 engine: the three uint8 [out, in/2] code matrices (int4.quantize_g128), `scales` ([out, in/128] of the engine's
         dtype, bfloat16 or float16) and `zeros` (uint8 [out, in/128])."""
         parts = self._quant_parts(tensors, scales, zeros)

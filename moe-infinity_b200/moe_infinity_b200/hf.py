@@ -1,7 +1,7 @@
 """HuggingFace plug-in helpers: run a `transformers` Mixtral, DeepSeek-V3, Qwen2-MoE, Qwen3-MoE or Llama 4 model with its MoE
 blocks executed by the CUDA engine (`patch_mixtral`, `patch_deepseek_v3`, `patch_qwen_moe`, `patch_llama4`), and load the
-routed experts of a published AWQ / GPTQ 4-bit checkpoint into an f16 int4 engine as they are stored
-(`load_int4_checkpoint`).
+routed experts of a published AWQ / GPTQ 4-bit checkpoint into an f16 int4 engine (`load_int4_checkpoint`) or of a published
+FP8 checkpoint into an fp8 engine (`load_fp8_checkpoint`) as they are stored.
 
 The reference achieves this by monkey-patching HF classes at load time (moe_infinity/runtime/model_offload.py:285-321:
 `MixtralSparseMoeBlock -> SyncMixtralSparseMoeBlock`).  The installed transformers (5.x) stores the experts of a layer as
@@ -25,11 +25,12 @@ from .engine import MoEEngine
 
 
 def _load(engine: MoEEngine, layer: int, expert: int, ws, resident: bool):
-    """Hand one expert's bf16 matrices to `engine`, quantised first when the engine stores fp8 (`fp8.quantize_block128`) or
-    int4 (`int4.quantize_g128`, with scales of the engine's dtype) experts."""
+    """Hand one expert's bf16 matrices to `engine`, quantised first when the engine stores fp8 (`fp8.quantize_block128`, or
+    `fp8.quantize_row` for fp8_scales="row") or int4 (`int4.quantize_g128`, with scales of the engine's dtype) experts."""
     kw = {}
     if engine.fp8:
-        ws, scales = zip(*[F8.quantize_block128(w) for w in ws])
+        quantize = F8.quantize_row if engine.fp8_scales == "row" else F8.quantize_block128
+        ws, scales = zip(*[quantize(w) for w in ws])
         kw = dict(scales=scales)
     elif engine.int4:
         ws, scales, zeros = zip(*[I4.quantize_g128(w, scale_dtype=engine.dtype) for w in ws])
@@ -418,4 +419,205 @@ def load_int4_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], q
             if not mixtral and engine.router == L.ROUTER_DEEPSEEK_V3:
                 key = f"{base}.gate.e_score_correction_bias"
                 engine.set_gate_bias(l, where[key].get_tensor(key).float())
+    return layers
+
+
+# ---------------------------------------------------------------- published FP8 checkpoints
+def _fp8_layout(qc: dict):
+    """Validate a checkpoint's `quantization_config`; return (quant_method, the engine's fp8_scales it loads into, the name
+    suffix of a linear layer's scale tensor)."""
+    method = str(qc.get("quant_method", "")).lower()
+    if method == "fbgemm_fp8":
+        return method, "row", "weight_scale"
+    if method != "fp8":
+        raise ValueError(f"quant_method {method!r}: only 'fbgemm_fp8' and 'fp8' checkpoints are supported")
+    fmt = str(qc.get("fmt", "e4m3")).lower()
+    if fmt != "e4m3":
+        raise ValueError(f"fp8 checkpoint with fmt={fmt!r}: only e4m3 weights are supported")
+    block = qc.get("weight_block_size")
+    if block is None:
+        return method, "row", "weight_scale_inv"               # one scale per tensor: the row format, scalar repeated
+    if list(block) != [F8.BLOCK, F8.BLOCK]:
+        raise ValueError(f"fp8 checkpoint with weight_block_size={list(block)}: only [{F8.BLOCK}, {F8.BLOCK}] blocks are supported")
+    return method, "block128", "weight_scale_inv"
+
+
+def _t8(q: torch.Tensor) -> torch.Tensor:
+    """The transpose of an e4m3 matrix, contiguous (the codes are moved, not converted)."""
+    return q.view(torch.uint8).t().contiguous().view(torch.float8_e4m3fn)
+
+
+def load_fp8_checkpoint(engine: MoEEngine, shards: Union[str, Sequence[str]], quantization_config: dict, model_type: str,
+                        resident: bool = True) -> List[int]:
+    """Load the routed experts, router weights and shared experts of a published FP8 checkpoint (its safetensors `shards`,
+    its config's `quantization_config`, `model_type` "mixtral", "qwen2_moe" / "qwen3_moe", "deepseek_v3" or "llama4") into
+    `engine`, an fp8 engine (`MoEEngine(dtype=torch.bfloat16, expert_dtype=torch.float8_e4m3fn, fp8_scales=...)`), without
+    changing a weight byte.  Tensors are read one at a time with `safetensors.safe_open`.
+
+    quant_method "fbgemm_fp8" (Llama 4 Maverick FP8, transformers' fbgemm quantiser): one fp32 scale per output channel,
+    loaded into an engine with fp8_scales="row".  Llama 4 stores a layer's experts fused and transposed:
+    feed_forward.experts.gate_up_proj e4m3 [E, H, 2I] with gate_up_proj_scale [E, 1, 2I] and down_proj [E, I, H] with
+    down_proj_scale [E, H, 1]; the router is feed_forward.router.weight; layers live under model.layers or
+    language_model.model.layers, and the MoE layers are the ones with a router.  Other models store one linear layer per
+    matrix: weight e4m3 [out, in] with weight_scale [out, 1].
+    quant_method "fp8" (transformers' fine-grained FP8): weight e4m3 with weight_scale_inv, which multiplies.  With
+    weight_block_size [128, 128] (DeepSeek-V3 / R1, Qwen3-MoE FP8) the scale is a [out/128, in/128] grid, loaded into a
+    block engine (fp8_scales="block128"); without a block size it is one scalar per tensor, loaded into a row engine with
+    the scalar repeated over the rows.
+    Names otherwise as `load_int4_checkpoint`: Mixtral model.layers.{l}.block_sparse_moe.experts.{e}.w{1,2,3} and
+    ...block_sparse_moe.gate.weight; DeepSeek / Qwen model.layers.{l}.mlp.experts.{e}.{gate,up,down}_proj, mlp.gate.weight
+    (layers without it are skipped), mlp.gate.e_score_correction_bias for a V3 router, and the Qwen shared-expert gate
+    mlp.shared_expert_gate.weight.  Shared experts (mlp.shared_experts, mlp.shared_expert, feed_forward.shared_expert) may
+    be stored plain or in FP8; either way they are registered dequantised to bf16.  `resident=False` registers the routed
+    experts as pinned host blobs (offload).
+    The engine then computes the bf16 layer on the dequantised weights (`fp8.dequantize_row` / `dequantize_block128`), not
+    the checkpoint's own forward with FP8 activations.
+    Refused with a message: other methods, formats or block sizes, a checkpoint whose scale layout does not match the
+    engine's fp8_scales, a model type that does not match the engine's expert type or router, dimensions that are not
+    multiples of 128, tensors of the wrong dtype or shape, and a missing tensor.  Returns the layers it loaded."""
+    from safetensors import safe_open
+
+    method, fmt, scale_name = _fp8_layout(quantization_config)
+    if not engine.fp8 or engine.dtype != torch.bfloat16:
+        raise ValueError("load_fp8_checkpoint needs an fp8 engine with bf16 activations "
+                         "(MoEEngine(dtype=torch.bfloat16, expert_dtype=torch.float8_e4m3fn))")
+    if engine.fp8_scales != fmt:
+        raise ValueError(f"this {method} checkpoint holds {'per-row' if fmt == 'row' else '128x128 block'} scales: it loads "
+                         f"into an engine with fp8_scales={fmt!r}, not {engine.fp8_scales!r}")
+    mixtral = model_type == "mixtral"
+    qwen = model_type in ("qwen2_moe", "qwen3_moe")
+    llama4 = model_type == "llama4"
+    if not (mixtral or qwen or llama4 or model_type.startswith("deepseek")):
+        raise ValueError(f"model_type {model_type!r}: Mixtral, Qwen-MoE, DeepSeek and Llama 4 checkpoints are supported")
+    if llama4 and method != "fbgemm_fp8":
+        raise ValueError(f"a Llama 4 checkpoint with quant_method {method!r}: only fbgemm_fp8 Llama 4 experts are supported")
+    if mixtral != (engine.expert_type == L.EXPERT_MIXTRAL):
+        raise ValueError(f"model_type {model_type!r} does not match the engine's expert_type {engine.expert_type}")
+    if qwen != (engine.router == L.ROUTER_QWEN_MOE) or llama4 != (engine.router == L.ROUTER_LLAMA4):
+        raise ValueError(f"model_type {model_type!r} does not match the engine's router {engine.router}")
+    H, I, E, Is = engine.H, engine.I, engine.E, engine.shared_inter
+    if H % F8.BLOCK or I % F8.BLOCK:
+        raise ValueError(f"hidden {H} and inter {I} must be multiples of {F8.BLOCK} for fp8 experts")
+    if isinstance(shards, str):
+        shards = [shards]
+    e4m3 = torch.float8_e4m3fn
+    with contextlib.ExitStack() as stack:
+        files = [stack.enter_context(safe_open(path, framework="pt", device="cpu")) for path in shards]
+        where: Dict[str, object] = {k: f for f in files for k in f.keys()}
+
+        def get(key: str) -> torch.Tensor:
+            return where[key].get_tensor(key)
+
+        def scales_of(key: str, s: torch.Tensor, rows: int, cols: int) -> torch.Tensor:
+            """The engine's scales of a [rows, cols] matrix from its checkpoint scale tensor `key` (fp32 values kept)."""
+            if s.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+                raise ValueError(f"{key}: scales must be floating point, got {s.dtype}")
+            s = s.float()                                          # (exact from bf16 / fp16)
+            if fmt == "block128":
+                if tuple(s.shape) != (rows // F8.BLOCK, cols // F8.BLOCK):
+                    raise ValueError(f"{key}: shape {tuple(s.shape)} is not the 128x128 block grid of a [{rows}, {cols}] matrix")
+                return s.contiguous()
+            if method == "fp8":                                    # per-tensor: one scalar
+                if s.numel() != 1:
+                    raise ValueError(f"{key}: shape {tuple(s.shape)} is not the single scale of a per-tensor checkpoint")
+                return s.reshape(1).expand(rows).contiguous()
+            if tuple(s.shape) not in ((rows,), (rows, 1)):
+                raise ValueError(f"{key}: shape {tuple(s.shape)} is not one scale per row of a [{rows}, {cols}] matrix")
+            return s.reshape(rows).contiguous()
+
+        def codes(key: str, q: torch.Tensor, shape) -> torch.Tensor:
+            if q.dtype != e4m3 or tuple(q.shape) != tuple(shape):
+                raise ValueError(f"{key}: expected float8_e4m3fn {tuple(shape)}, got {q.dtype} {tuple(q.shape)}")
+            return q
+
+        def linear(prefix: str, rows: int, cols: int):
+            """(q, s) of one per-matrix FP8 linear layer."""
+            q = codes(f"{prefix}.weight", get(f"{prefix}.weight"), (rows, cols))
+            key = f"{prefix}.{scale_name}"
+            return q, scales_of(key, get(key), rows, cols)
+
+        def dequantize(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+            return F8.dequantize_row(q, s) if fmt == "row" else F8.dequantize_block128(q, s)
+
+        def shared(prefix: str, rows: int, cols: int) -> torch.Tensor:
+            """A shared expert's linear layer in bf16: stored plain, or FP8 dequantised."""
+            w = get(f"{prefix}.weight")
+            if tuple(w.shape) != (rows, cols):
+                raise ValueError(f"{prefix}.weight: expected shape {(rows, cols)}, got {tuple(w.shape)}")
+            if w.dtype != e4m3:
+                return w.to(engine.dtype)
+            key = f"{prefix}.{scale_name}"
+            if key not in where:
+                raise ValueError(f"the checkpoint has no tensor {key} (the scale of the FP8 {prefix}.weight)")
+            return dequantize(w, scales_of(key, get(key), rows, cols))
+
+        if llama4:
+            root = next((r for r in ("model.layers", "language_model.model.layers")
+                         if any(f"{r}.{l}.feed_forward.router.weight" in where for l in range(engine.L))), None)
+            if root is None:
+                raise ValueError("the checkpoint has no Llama 4 MoE layer (no {model.,language_model.model.}layers.*"
+                                 ".feed_forward.router.weight)")
+            layers = [l for l in range(engine.L) if f"{root}.{l}.feed_forward.router.weight" in where]
+            moe, router, shared_name = "feed_forward", "router", "shared_expert"
+            names = ("gate_proj", "up_proj", "down_proj")
+        elif mixtral:
+            root, moe, router, shared_name = "model.layers", "block_sparse_moe", "gate", None
+            layers = list(range(engine.L))
+            names = ("w1", "w2", "w3")                                 # reference order: w1 | w2 | w3
+        else:
+            root, moe, router = "model.layers", "mlp", "gate"
+            shared_name = "shared_expert" if qwen else "shared_experts"
+            layers = [l for l in range(engine.L) if f"{root}.{l}.mlp.gate.weight" in where]
+            names = ("gate_proj", "up_proj", "down_proj")              # DeepSeek order: gate | up | down
+        shapes = {"w1": (I, H), "w2": (H, I), "w3": (I, H), "gate_proj": (I, H), "up_proj": (I, H), "down_proj": (H, I)}
+        shared_shapes = {"gate_proj": (Is, H), "up_proj": (Is, H), "down_proj": (H, Is)}
+        need = []
+        for l in layers:
+            base = f"{root}.{l}.{moe}"
+            need.append(f"{base}.{router}.weight")
+            if llama4:
+                need += [f"{base}.experts.{n}{p}" for n in ("gate_up_proj", "down_proj") for p in ("", "_scale")]
+            else:
+                need += [f"{base}.experts.{e}.{n}.{p}" for e in range(E) for n in names for p in ("weight", scale_name)]
+            if shared_name and Is > 0:
+                need += [f"{base}.{shared_name}.{n}.weight" for n in names]
+            if qwen and Is > 0:
+                need.append(f"{base}.shared_expert_gate.weight")
+            if engine.router == L.ROUTER_DEEPSEEK_V3:
+                need.append(f"{base}.gate.e_score_correction_bias")
+        missing = [k for k in need if k not in where]
+        if missing:
+            raise ValueError(f"the checkpoint has no tensor {missing[0]} ({len(missing)} missing)")
+        for l in layers:
+            base = f"{root}.{l}.{moe}"
+            if llama4:
+                # Llama4TextExperts computes x @ gate_up_proj[e]: column j of [H, 2I] is output channel j, scaled by
+                # gate_up_proj_scale[e, 0, j]; the engine takes the nn.Linear [out, in] transposes
+                k_gu, k_dn = f"{base}.experts.gate_up_proj", f"{base}.experts.down_proj"
+                gu, dn = codes(k_gu, get(k_gu), (E, H, 2 * I)), codes(k_dn, get(k_dn), (E, I, H))
+                gus, dns = get(f"{k_gu}_scale"), get(f"{k_dn}_scale")
+                if tuple(gus.shape) != (E, 1, 2 * I) or tuple(dns.shape) != (E, H, 1):
+                    raise ValueError(f"{k_gu}_scale / {k_dn}_scale: shapes {tuple(gus.shape)} / {tuple(dns.shape)} are not "
+                                     f"per-output-channel scales {(E, 1, 2 * I)} / {(E, H, 1)}")
+
+                def expert(e):
+                    return [(_t8(gu[e][:, :I]), scales_of(f"{k_gu}_scale", gus[e, 0, :I], I, H)),
+                            (_t8(gu[e][:, I:]), scales_of(f"{k_gu}_scale", gus[e, 0, I:], I, H)),
+                            (_t8(dn[e]), scales_of(f"{k_dn}_scale", dns[e, :, 0], H, I))]
+            else:
+                def expert(e):
+                    return [linear(f"{base}.experts.{e}.{n}", *shapes[n]) for n in names]
+            for e in range(E):
+                qs, ss = zip(*expert(e))
+                if resident:
+                    engine.load_expert(l, e, qs, scales=ss)
+                else:
+                    engine.register_expert(l, e, qs, scales=ss)
+            if shared_name and Is > 0:
+                engine.register_shared(l, [shared(f"{base}.{shared_name}.{n}", *shared_shapes[n]) for n in names])
+            if qwen and Is > 0:
+                engine.set_shared_gate(l, get(f"{base}.shared_expert_gate.weight").to(engine.dtype))
+            engine.set_gate(l, get(f"{base}.{router}.weight"))
+            if engine.router == L.ROUTER_DEEPSEEK_V3:
+                engine.set_gate_bias(l, get(f"{base}.gate.e_score_correction_bias").float())
     return layers
